@@ -419,6 +419,9 @@ typedef struct {
     int32_t ell_col_bytes;                        /* HELL: bytes per ELL slot of the column encoding: 4 = 32-bit columns,
                                                      2 = 16-bit offsets ("spmv.col16"), 0 = no column array, one slot mask
                                                      byte per row ("spmv.ell_diag"; width 0 also reports 0) */
+    int32_t ell_classes;                          /* HELL: number of row classes ("spmv.ell_classes": one class byte per row,
+                                                     slot masks and values in a table of at most 256 classes); 0 = values
+                                                     stored per slot */
 } vexb_spmat_info;
 int vexb_spmat_get_info(const vexb_spmat *A, vexb_spmat_info *info);
 /* Copy the HELL arrays back (parity with hybrid_ell.inl:132-193); any pointer may be NULL. */

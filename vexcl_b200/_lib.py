@@ -53,7 +53,8 @@ class SpmatInfo(C.Structure):
     _fields_ = [("nrows", C.c_size_t), ("ncols", C.c_size_t), ("nnz", C.c_size_t), ("fmt", C.c_int32),
                 ("val_dtype", C.c_int32), ("ell_width", C.c_size_t), ("ell_pitch", C.c_size_t),
                 ("csr_tail_nnz", C.c_size_t), ("n_tiles", C.c_size_t), ("tile_nnz", C.c_size_t),
-                ("device_bytes", C.c_size_t), ("ell_col_bytes", C.c_int32)]
+                ("device_bytes", C.c_size_t), ("ell_col_bytes", C.c_int32),
+                ("ell_classes", C.c_int32)]
 
 
 class CcsrInfo(C.Structure):

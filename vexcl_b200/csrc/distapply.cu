@@ -62,7 +62,7 @@ struct DistArgs {
     int rank, nparts;
     const int4 *push_blk; const int *send_cols; int n_push_blocks;
     // interior strip (hybrid ELL)
-    size_t n_int, pitch; int w_dyn; EllShifts shift; const void *ell_col /* vexb_spmat::ell_col_any() */; const T *ell_val;
+    size_t n_int, pitch; int w_dyn; EllShifts shift; const void *ell_col /* vexb_spmat::ell_col_any() */; const T *ell_val /* ell_val_any() */;
     const int *tail_ptr, *tail_col; const T *tail_val; const int *int_row_ids; size_t y_off; int n_int_blocks;
     // boundary rows
     size_t b_n, b_pitch; int b_w; const int *b_col; const T *b_val; const int *b_rows; int n_bnd_blocks;
@@ -92,8 +92,11 @@ __device__ __forceinline__ bool wait_flag(const unsigned long long *flag, unsign
 }
 
 // dot partials: one value per block in dot_ws (own buffer, not the Reductor workspace)
+// Register bound: 32 per thread (8 blocks per SM).  Row-class strips get 40 (6 blocks per SM): under 32 their row body,
+// which keeps all W gathers of x in flight before the class byte returns (hell_class_rows), spilled 24 bytes at every
+// width, in the interior rows as well as the boundary rows.
 template <class T, int W, class C, bool DOT>
-__global__ void __launch_bounds__(256, 8) dist_apply_kernel(const __grid_constant__ DistArgs<T> a) {
+__global__ void __launch_bounds__(256, std::is_same<C, EllClass>::value ? 6 : 8) dist_apply_kernel(const __grid_constant__ DistArgs<T> a) {
     unsigned long long *mine = a.box[a.rank];
     __shared__ unsigned long long s_epoch;
     __shared__ int s_ok;
@@ -445,7 +448,14 @@ static int launch_dist(const vexb_dspmat *A, cudaStream_t st, const DistArgs<T> 
     const size_t w = hell ? S->ell_width : 0;
 #define DL(W) do { if (hell && S->ell_col16) dist_apply_kernel<T, W, short, DOT><<<grid, 256, 0, st>>>(a); \
                    else dist_apply_kernel<T, W, int, DOT><<<grid, 256, 0, st>>>(a); } while (0)
-    if (hell && S->ell_mask) {
+    if (hell && S->ell_class) {
+        switch (w) {   // = the widths spmv.cu build() gives row classes
+            case 5: dist_apply_kernel<T, 5, EllClass, DOT><<<grid, 256, 0, st>>>(a); break;
+            case 7: dist_apply_kernel<T, 7, EllClass, DOT><<<grid, 256, 0, st>>>(a); break;
+            case 3: dist_apply_kernel<T, 3, EllClass, DOT><<<grid, 256, 0, st>>>(a); break;
+            default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no dist_apply_kernel for row classes of width %zu", w);
+        }
+    } else if (hell && S->ell_mask) {
         switch (w) {   // = the widths spmv.cu build() gives slot masks
             case 5: dist_apply_kernel<T, 5, EllDiag, DOT><<<grid, 256, 0, st>>>(a); break;
             case 7: dist_apply_kernel<T, 7, EllDiag, DOT><<<grid, 256, 0, st>>>(a); break;
@@ -489,7 +499,7 @@ static int dist_apply_t(const vexb_dspmat *A, cudaStream_t st, const T *x, T *y,
     const bool fused_interior = S && S->fmt == VEXB_FMT_HELL && S->nnz > 0 && S->nrows_stored > 0;
     if (fused_interior) {
         a.n_int = S->nrows_stored; a.pitch = S->ell_pitch; a.w_dyn = (int)S->ell_width; a.shift = S->ell_shifts;
-        a.ell_col = S->ell_col_any(); a.ell_val = (const T *)S->ell_val;
+        a.ell_col = S->ell_col_any(); a.ell_val = (const T *)S->ell_val_any();
         a.tail_ptr = S->tail_ptr; a.tail_col = S->tail_col; a.tail_val = (const T *)S->tail_val;
         a.int_row_ids = S->row_ids; a.y_off = S->y_offset;
         a.n_int_blocks = (int)((S->nrows_stored + 255) / 256);

@@ -8,7 +8,8 @@ namespace vexb {
 // has its neighbours n*n, n, 1 away -- no single shift brings them all within 16 bits, one shift per slot does).  Slots
 // past the last entry share it.
 constexpr int kEllShiftSlots = 16;
-struct EllShifts { int s[kEllShiftSlots]; };
+// x_max: largest column the strip stores, set on row-class strips only (EllClass below).
+struct EllShifts { int s[kEllShiftSlots]; int x_max; };
 // Widths for which EVERY kernel that walks an ELL strip has an unrolled instantiation (hell_kernel, hell_multi_kernel,
 // dist_apply_kernel: keep their switches in step with this).  Only those strips get one shift per slot: the kernels'
 // run-time loop over the slots reads shift.s[0] for all of them (indexing the by-value table at run time spills it).
@@ -18,6 +19,13 @@ constexpr bool ell_width_is_unrolled_everywhere(size_t w) { return w == 3 || w =
 // per-row masks where the other encodings pass their column array.
 constexpr size_t kEllDiagMaxWidth = 8;
 struct EllDiag { unsigned char mask; };
+// Column type of the fourth ELL encoding (spmv.ell_classes): a slot-mask strip whose rows take at most kEllMaxClasses
+// distinct (slot mask, W slot values) tuples -- any constant-coefficient stencil -- stores one class byte per row and no
+// per-slot values.  The kernels take the class bytes where they take masks and the class table where they take the
+// values.  Class table, in device memory: kEllClassHeader bytes of slot masks (one per class), then W values per class.
+constexpr size_t kEllMaxClasses = 256;
+constexpr size_t kEllClassHeader = 256;
+struct EllClass { unsigned char id; };
 }
 
 struct vexb_spmat {
@@ -37,8 +45,13 @@ struct vexb_spmat {
     int *ell_col = nullptr; void *ell_val = nullptr;
     short *ell_col16 = nullptr; vexb::EllShifts ell_shifts = {};   // optional: columns as 16-bit offsets from (row + shift of the slot); see spmv.col16
     vexb::EllDiag *ell_mask = nullptr;   // optional: one slot mask per stored row, column of slot k = row + ell_shifts.s[k]; see spmv.ell_diag
-    // exactly one of ell_col / ell_col16 / ell_mask is set on a HELL strip of width > 0
-    const void *ell_col_any() const { return ell_mask ? (const void *)ell_mask : ell_col16 ? (const void *)ell_col16 : (const void *)ell_col; }
+    // optional: one class id per stored row and the class table in place of ell_mask and ell_val; see spmv.ell_classes
+    vexb::EllClass *ell_class = nullptr; void *ell_ctab = nullptr; size_t ell_nclass = 0;
+    // exactly one of ell_col / ell_col16 / ell_mask / ell_class is set on a HELL strip of width > 0
+    const void *ell_col_any() const {
+        return ell_class ? (const void *)ell_class : ell_mask ? (const void *)ell_mask : ell_col16 ? (const void *)ell_col16 : (const void *)ell_col;
+    }
+    const void *ell_val_any() const { return ell_class ? ell_ctab : ell_val; }
     int *tail_ptr = nullptr; int *tail_col = nullptr; void *tail_val = nullptr;
     // SELL-32-sigma: slice s holds stored rows perm[32 s .. 32 s + 31] (-1: none) in sell_col / sell_val at
     // [slice_ptr[s], slice_ptr[s+1]), slot k of lane l at slice_ptr[s] + 32 k + l
@@ -57,10 +70,11 @@ struct vexb_spmat {
 namespace vexb {
 // Everything a kernel generated for a VEXB_TERM_SPMV terminal reads about the strip (uniform loads through one pointer).
 struct SpmvDesc {
-    const void *ell_col;   // vexb_spmat::ell_col_any(): 32-bit columns, 16-bit offsets or slot masks
-    const void *ell_val; const int *tail_ptr; const int *tail_col; const void *tail_val;
+    const void *ell_col;   // vexb_spmat::ell_col_any(): 32-bit columns, 16-bit offsets, slot masks or class ids
+    const void *ell_val;   // vexb_spmat::ell_val_any(): values, or the class table
+    const int *tail_ptr; const int *tail_col; const void *tail_val;
     const int *rowptr; const int *col; const void *val;
-    unsigned long long pitch; int width; int shifts[kEllShiftSlots];
+    unsigned long long pitch; int width; int shifts[kEllShiftSlots]; int x_max;
 };
 }
 

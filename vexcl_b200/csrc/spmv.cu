@@ -471,17 +471,38 @@ __global__ void __launch_bounds__(kPipeThreads) csr_pipe_kernel(const int2 *__re
     }
 }
 
+// Rows per thread of hell_kernel on row-class strips.  Measured on configs[2] / configs[3] (H100 80GB HBM3, 400 W):
+// 1 row 0.080 / 0.137 ms, 2 rows 0.077 / 0.126 ms, 4 rows 0.083 / 0.140 ms.
+constexpr int kEllClassRows = 2;
+
 template <class T, int W, class C>
 __global__ void __launch_bounds__(256) hell_kernel(size_t n, size_t pitch, int w_dyn, const C *__restrict__ ell_col, const EllShifts shift,
                                                     const T *__restrict__ ell_val, const int *__restrict__ tail_ptr,
                                                     const int *__restrict__ tail_col, const T *__restrict__ tail_val,
                                                     const T *__restrict__ x, T *y, T alpha, int append,
                                                     const int *__restrict__ row_ids) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
-    const T sum = hell_row_sum<T, W, C>(i, pitch, w_dyn, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep);
-    store_y<T>(y, row_ids ? (size_t)row_ids[i] : i, sum, alpha, append);
+    if constexpr (std::is_same<C, EllClass>::value) {
+        // Row classes: a row moves 17 bytes (class, x, y), too few for one row per thread to keep enough bytes in flight.
+        // A thread takes kEllClassRows rows, a block apart, so at every sub-step a warp's lanes hold consecutive rows
+        // (coalesced class bytes and y stores); rows past the end repeat row n-1 and store nothing.
+        constexpr int R = kEllClassRows;
+        const size_t i0 = (size_t)blockIdx.x * blockDim.x * R + threadIdx.x;
+        if (i0 >= n) return;
+        const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+        size_t rows[R]; T sum[R];
+#pragma unroll
+        for (int r = 0; r < R; ++r) rows[r] = min(i0 + (size_t)r * blockDim.x, n - 1);
+        hell_class_rows<T, W, R>(rows, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep, sum);
+#pragma unroll
+        for (int r = 0; r < R; ++r)
+            if (i0 + (size_t)r * blockDim.x < n) store_y<T>(y, row_ids ? (size_t)row_ids[rows[r]] : rows[r], sum[r], alpha, append);
+    } else {
+        const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+        if (i >= n) return;
+        const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+        const T sum = hell_row_sum<T, W, C>(i, pitch, w_dyn, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep);
+        store_y<T>(y, row_ids ? (size_t)row_ids[i] : i, sum, alpha, append);
+    }
 }
 
 // ---- several right-hand sides at once: SpMat * multivector (vexcl/multivector.hpp, operations.hpp:861-881) ------------
@@ -504,29 +525,53 @@ __global__ void __launch_bounds__(256) hell_multi_kernel(size_t n, size_t pitch,
 #pragma unroll
     for (int k = 0; k < K; ++k) sum[k] = T(0);
     static_assert(W > 0 || !std::is_same<C, EllDiag>::value, "the diagonal encoding needs one shift per slot: unrolled widths only");
-    const unsigned mask = ell_row_mask(ell_col, i, stream);
-    if (W > 0) {
-        int c[W > 0 ? W : 1]; T v[W > 0 ? W : 1];
+    if constexpr (std::is_same<C, EllClass>::value) {
+        // row classes (hell_class_rows): the first component's gathers go out before the class byte is back; the
+        // row's mask and values are then looked up once for all K components
+        static_assert(W > 0 && W <= (int)kEllDiagMaxWidth, "row classes hold one slot mask byte: unrolled widths up to 8 only");
+        const unsigned id = ldg_stream(ell_col + i, stream);
+        T xv[W];
 #pragma unroll
-        for (int j = 0; j < W; ++j) { c[j] = ell_slot_column(ell_col, i, pitch, j, ell_shift_of(shift, j), mask, stream); v[j] = ldg_stream(ell_val + i + (size_t)j * pitch, stream); }
-        // one component at a time (W gathers in flight, then that component's products), the order chosen over issuing
-        // all K*W gathers first
+        for (int j = 0; j < W; ++j) xv[j] = ldg_keep(static_cast<const T *>(mp.x[0]) + ell_class_column(i, shift, j), keep);
+        const unsigned m = ldg_table(reinterpret_cast<const unsigned char *>(ell_val) + id);
+        T v[W];
+#pragma unroll
+        for (int j = 0; j < W; ++j) v[j] = ldg_table(ell_val + kEllClassHeader / sizeof(T) + id * W + j);
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            const T *x = static_cast<const T *>(mp.x[k]);
-            T xv[W > 0 ? W : 1];
+            if (k > 0) {
+                const T *x = static_cast<const T *>(mp.x[k]);
 #pragma unroll
-            for (int j = 0; j < W; ++j) xv[j] = (c[j] != -1) ? ldg_keep(x + c[j], keep) : T(0);
+                for (int j = 0; j < W; ++j) xv[j] = ldg_keep(x + ell_class_column(i, shift, j), keep);
+            }
 #pragma unroll
-            for (int j = 0; j < W; ++j) if (c[j] != -1) sum[k] = t_add<T>(sum[k], t_mul<T>(v[j], xv[j]));
+            for (int j = 0; j < W; ++j) if ((m >> j) & 1u) sum[k] = t_add<T>(sum[k], t_mul<T>(v[j], xv[j]));
         }
     } else {
-        for (int j = 0; j < w_dyn; ++j) {
-            const int c = ell_slot_column(ell_col, i, pitch, j, shift.s[0], mask, stream);   // run-time widths: one shift for all slots (build())
-            if (c != -1) {
-                const T v = ldg_stream(ell_val + i + (size_t)j * pitch, stream);
+        const unsigned mask = ell_row_mask(ell_col, i, stream);
+        if (W > 0) {
+            int c[W > 0 ? W : 1]; T v[W > 0 ? W : 1];
 #pragma unroll
-                for (int k = 0; k < K; ++k) sum[k] = t_add<T>(sum[k], t_mul<T>(v, ldg_keep(static_cast<const T *>(mp.x[k]) + c, keep)));
+            for (int j = 0; j < W; ++j) { c[j] = ell_slot_column(ell_col, i, pitch, j, ell_shift_of(shift, j), mask, stream); v[j] = ldg_stream(ell_val + i + (size_t)j * pitch, stream); }
+            // one component at a time (W gathers in flight, then that component's products), the order chosen over issuing
+            // all K*W gathers first
+#pragma unroll
+            for (int k = 0; k < K; ++k) {
+                const T *x = static_cast<const T *>(mp.x[k]);
+                T xv[W > 0 ? W : 1];
+#pragma unroll
+                for (int j = 0; j < W; ++j) xv[j] = (c[j] != -1) ? ldg_keep(x + c[j], keep) : T(0);
+#pragma unroll
+                for (int j = 0; j < W; ++j) if (c[j] != -1) sum[k] = t_add<T>(sum[k], t_mul<T>(v[j], xv[j]));
+            }
+        } else {
+            for (int j = 0; j < w_dyn; ++j) {
+                const int c = ell_slot_column(ell_col, i, pitch, j, shift.s[0], mask, stream);   // run-time widths: one shift for all slots (build())
+                if (c != -1) {
+                    const T v = ldg_stream(ell_val + i + (size_t)j * pitch, stream);
+#pragma unroll
+                    for (int k = 0; k < K; ++k) sum[k] = t_add<T>(sum[k], t_mul<T>(v, ldg_keep(static_cast<const T *>(mp.x[k]) + c, keep)));
+                }
             }
         }
     }
@@ -952,6 +997,36 @@ static bool find_row_patterns(size_t n, const std::vector<int> &rowptr, const st
     return true;
 }
 
+// Row classes of a slot-mask strip (spmv.ell_classes): the distinct (slot mask, W slot values) tuples of its `pitch`
+// stored rows -- padding rows included, which give the mask-0 tuple -- numbered in order of first appearance.  Fills
+// id (one class per row) and the class table as the kernels read it (kEllClassHeader bytes of masks, then W values per
+// class), and returns the number of classes; 0 when there are more than kEllMaxClasses.  Values are compared bit for bit.
+template <class T>
+static size_t ell_row_classes(size_t pitch, size_t w, const std::vector<EllDiag> &mask, const std::vector<T> &eval,
+                              std::vector<unsigned char> &id, std::vector<unsigned char> &table) {
+    const size_t tb = w * sizeof(T);
+    id.assign(pitch, 0); table.assign(kEllClassHeader, 0);
+    std::unordered_map<std::string, int> seen;
+    std::string key(1 + tb, '\0');
+    int last = -1;
+    for (size_t i = 0; i < pitch; ++i) {
+        key[0] = (char)mask[i].mask;
+        for (size_t k = 0; k < w; ++k) std::memcpy(&key[1 + k * sizeof(T)], &eval[i + pitch * k], sizeof(T));
+        if (last >= 0 && table[last] == (unsigned char)key[0] &&                      // most rows repeat the previous row's class
+            std::memcmp(&table[kEllClassHeader + (size_t)last * tb], &key[1], tb) == 0) { id[i] = (unsigned char)last; continue; }
+        auto it = seen.find(key);
+        if (it == seen.end()) {
+            if (seen.size() == kEllMaxClasses) return 0;
+            const int c = (int)seen.size();
+            table[c] = (unsigned char)key[0];
+            table.insert(table.end(), key.begin() + 1, key.end());
+            it = seen.emplace(key, c).first;
+        }
+        id[i] = (unsigned char)(last = it->second);
+    }
+    return seen.size();
+}
+
 template <class T>
 static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col, std::vector<T> &val, int fmt, bool plain) {
     const size_t n = A->nrows_stored;
@@ -1151,7 +1226,6 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
             tptr[i + 1] = (int)tcol.size();
         }
         A->tail_nnz = tcol.size();
-        VEXB_TRY(upload(eval, 0, &A->ell_val, &A->device_bytes));
         if (param("spmv.col16", 1) && w > 0) {
             // Banded matrices: the stored columns of ELL slot k lie within +-32767 of (row + shift[k]) for one shift per
             // slot, so the ELL columns fit 16 bits.  The kernel then streams 10 instead of 12 bytes per stored entry; same
@@ -1181,16 +1255,34 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
                 // array carries no information beyond which slots are padding.  Store that as one mask byte per row and
                 // the distances themselves as the shifts: 8 + 1/w instead of 10 bytes per stored entry, same bits in y.
                 // spmv.ell_diag = 0 stops at 16-bit columns.
-                EllShifts sh;
+                EllShifts sh{};
                 for (int g = 0; g < kEllShiftSlots; ++g) sh.s[g] = any[g] ? (int)lo[g] : 0;
                 std::vector<EllDiag> mask(pitch, EllDiag{0});
                 for (size_t k = 0; k < w; ++k)
                     for (size_t i = 0; i < n; ++i)
                         if (ecol[i + pitch * k] >= 0) mask[i].mask |= (unsigned char)(1u << k);
                 A->ell_shifts = sh;
-                VEXB_TRY(upload(mask, 0, (void **)&A->ell_mask, &A->device_bytes));
+                // Row classes: a constant-coefficient stencil has a handful of distinct rows (2 on a 5-point Laplacian:
+                // interior and identity), so one class byte per row and a small table of masks and values replace the
+                // masks and the W values per row -- 17 instead of 57 bytes per row of configs[2] moved by a product.
+                // spmv.ell_classes: 0 = never, 1 (default) = when the values would exceed the L2, 2 = at any size.
+                // Smaller strips keep slot masks and their stored layout (DESIGN.md section 3 has the measurement
+                // below the floor).
+                const long classes = param("spmv.ell_classes", 1);
+                int l2 = 0;
+                if (classes == 1) VEXB_CUDA(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, A->dev));
+                std::vector<unsigned char> cid, ctab;
+                if ((classes == 2 || (classes == 1 && eval.size() * sizeof(T) > (size_t)l2)) &&
+                    (A->ell_nclass = ell_row_classes(pitch, w, mask, eval, cid, ctab)) > 0) {
+                    // padding slots gather x at a column clamped to the strip's largest one (ell_class_column)
+                    A->ell_shifts.x_max = *std::max_element(ecol.begin(), ecol.end());
+                    VEXB_TRY(upload(cid, 0, (void **)&A->ell_class, &A->device_bytes));
+                    VEXB_TRY(upload(ctab, 0, &A->ell_ctab, &A->device_bytes));
+                } else {
+                    VEXB_TRY(upload(mask, 0, (void **)&A->ell_mask, &A->device_bytes));
+                }
             } else if (fits && ok) {
-                EllShifts sh;
+                EllShifts sh{};
                 for (int g = 0; g < kEllShiftSlots; ++g) sh.s[g] = any[per_slot ? g : 0] ? (int)(lo[per_slot ? g : 0] + 32767) : 0;
                 std::vector<short> e16(pitch * w, (short)-32768);
                 for (size_t k = 0; k < w; ++k) {
@@ -1204,7 +1296,8 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
                 VEXB_TRY(upload(e16, 0, (void **)&A->ell_col16, &A->device_bytes));
             }
         }
-        if (!A->ell_col16 && !A->ell_mask) VEXB_TRY(upload(ecol, 0, (void **)&A->ell_col, &A->device_bytes));
+        if (!A->ell_col16 && !A->ell_mask && !A->ell_class) VEXB_TRY(upload(ecol, 0, (void **)&A->ell_col, &A->device_bytes));
+        if (!A->ell_class) VEXB_TRY(upload(eval, 0, &A->ell_val, &A->device_bytes));
         if (A->tail_nnz) {
             VEXB_TRY(upload(tptr, 0, (void **)&A->tail_ptr, &A->device_bytes));
             VEXB_TRY(upload(tcol, 0, (void **)&A->tail_col, &A->device_bytes));
@@ -1340,7 +1433,15 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
                   (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids); } while (0)
 #define HD(W) hell_kernel<T, W, EllDiag><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_mask, A->ell_shifts, \
                   (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids)
-        if (A->ell_mask) {
+#define HC(W) hell_kernel<T, W, EllClass><<<(unsigned)((n + 256 * kEllClassRows - 1) / (256 * kEllClassRows)), 256, 0, st>>>( \
+                  n, A->ell_pitch, (int)A->ell_width, A->ell_class, A->ell_shifts, (const T *)A->ell_ctab, A->tail_ptr, A->tail_col, \
+                  (const T *)A->tail_val, x, y, alpha, append, A->row_ids)
+        if (A->ell_class) {
+            switch (A->ell_width) {   // = the widths build() gives row classes: those of slot masks
+                case 3: HC(3); break; case 5: HC(5); break; case 7: HC(7); break;
+                default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no hell_kernel for row classes of width %zu", A->ell_width);
+            }
+        } else if (A->ell_mask) {
             switch (A->ell_width) {   // = the widths build() gives slot masks: ell_width_is_unrolled_everywhere and <= kEllDiagMaxWidth
                 case 3: HD(3); break; case 5: HD(5); break; case 7: HD(7); break;
                 default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no hell_kernel for slot masks of width %zu", A->ell_width);
@@ -1351,6 +1452,7 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
             case 9: HL(9); break;
             default: HL(0); break;
         }
+#undef HC
 #undef HD
 #undef HL
         VEXB_LAUNCHED();
@@ -1371,7 +1473,14 @@ static int spmv_multi_launch(const vexb_spmat *A, cudaStream_t st, const void *c
               (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, mp, alpha, append, A->row_ids, A->y_offset); } while (0)
 #define HD(W) hell_multi_kernel<T, W, EllDiag, K><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_mask, A->ell_shifts, \
               (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, mp, alpha, append, A->row_ids, A->y_offset)
-    if (A->ell_mask) {
+#define HC(W) hell_multi_kernel<T, W, EllClass, K><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_class, A->ell_shifts, \
+              (const T *)A->ell_ctab, A->tail_ptr, A->tail_col, (const T *)A->tail_val, mp, alpha, append, A->row_ids, A->y_offset)
+    if (A->ell_class) {
+        switch (A->ell_width) {   // = the widths build() gives row classes
+            case 3: HC(3); break; case 5: HC(5); break; case 7: HC(7); break;
+            default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no hell_multi_kernel for row classes of width %zu", A->ell_width);
+        }
+    } else if (A->ell_mask) {
         switch (A->ell_width) {   // = the widths build() gives slot masks
             case 3: HD(3); break; case 5: HD(5); break; case 7: HD(7); break;
             default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no hell_multi_kernel for slot masks of width %zu", A->ell_width);
@@ -1380,6 +1489,7 @@ static int spmv_multi_launch(const vexb_spmat *A, cudaStream_t st, const void *c
         case 3: HM(3); break; case 5: HM(5); break; case 7: HM(7); break; case 9: HM(9); break;   // = ell_width_is_unrolled_everywhere
         default: HM(0); break;
     }
+#undef HC
 #undef HD
 #undef HM
     VEXB_LAUNCHED();
@@ -1404,11 +1514,12 @@ int vexb::spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &
     }
     if (st == VEXB_OK && (A->fmt == VEXB_FMT_CSR || A->fmt == VEXB_FMT_HELL)) {
         SpmvDesc d; memset(&d, 0, sizeof(d));
-        d.ell_col = A->ell_col_any(); d.ell_val = A->ell_val;
+        d.ell_col = A->ell_col_any(); d.ell_val = A->ell_val_any();
         d.tail_ptr = A->tail_ptr; d.tail_col = A->tail_col; d.tail_val = A->tail_val;
         d.rowptr = A->rowptr; d.col = A->col; d.val = A->val;
         d.pitch = A->ell_pitch; d.width = (int)A->ell_width;
         for (int g = 0; g < kEllShiftSlots; ++g) d.shifts[g] = A->ell_shifts.s[g];
+        d.x_max = A->ell_shifts.x_max;
         cudaError_t e = cudaMalloc(&A->d_desc, sizeof(d));
         if (e == cudaSuccess) e = cudaMemcpy(A->d_desc, &d, sizeof(d), cudaMemcpyHostToDevice);
         if (e != cudaSuccess) { set_error(__FILE__, __LINE__, "strip descriptor upload failed: %s", cudaGetErrorString(e)); st = VEXB_ERR_CUDA; }
@@ -1479,7 +1590,7 @@ extern "C" int vexb_spmat_destroy(vexb_spmat *A) {
     cudaFree(A->val); cudaFree(A->col); cudaFree(A->rowptr); cudaFree(A->tile); cudaFree(A->tile_x); cudaFree(A->wtile); cudaFree(A->d_desc);
     vexb_ccsr_destroy(A->patterns);
     cudaFree(A->sell_ptr); cudaFree(A->sell_perm); cudaFree(A->sell_col); cudaFree(A->sell_col16); cudaFree(A->sell_val);
-    cudaFree(A->row_ids); cudaFree(A->ell_col); cudaFree(A->ell_col16); cudaFree(A->ell_mask); cudaFree(A->ell_val); cudaFree(A->tail_ptr); cudaFree(A->tail_col); cudaFree(A->tail_val);
+    cudaFree(A->row_ids); cudaFree(A->ell_col); cudaFree(A->ell_col16); cudaFree(A->ell_mask); cudaFree(A->ell_class); cudaFree(A->ell_ctab); cudaFree(A->ell_val); cudaFree(A->tail_ptr); cudaFree(A->tail_col); cudaFree(A->tail_val);
     delete A;
     return VEXB_OK;
 }
@@ -1492,7 +1603,8 @@ extern "C" int vexb_spmat_get_info(const vexb_spmat *A, vexb_spmat_info *info) {
     info->ell_width = A->ell_width; info->ell_pitch = A->ell_pitch; info->csr_tail_nnz = A->tail_nnz;
     info->n_tiles = A->n_tiles; info->tile_nnz = A->tile_nnz;
     info->device_bytes = A->device_bytes;
-    info->ell_col_bytes = A->ell_mask ? 0 : A->ell_col16 ? 2 : A->ell_col ? 4 : 0;
+    info->ell_col_bytes = A->ell_mask || A->ell_class ? 0 : A->ell_col16 ? 2 : A->ell_col ? 4 : 0;
+    info->ell_classes = (int32_t)A->ell_nclass;
     if (A->patterns) {
         vexb_ccsr_info ci;
         VEXB_TRY(vexb_ccsr_get_info(A->patterns, &ci));
@@ -1534,10 +1646,18 @@ extern "C" int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, v
     DeviceGuard g(A->dev);
     const size_t vs = dtype_size(A->val_dtype), ne = A->ell_pitch * A->ell_width;
     if (ell_col && ne && A->ell_col) VEXB_CUDA(cudaMemcpy(ell_col, A->ell_col, ne * 4, cudaMemcpyDeviceToHost));
-    if (ell_col && ne && A->ell_mask) {
+    // row classes: each row's mask and values are its class's entry in the table
+    std::vector<unsigned char> cid, ctab;
+    if ((ell_col || ell_val) && ne && A->ell_class) {
+        cid.resize(A->ell_pitch); ctab.resize(kEllClassHeader + A->ell_nclass * A->ell_width * vs);
+        VEXB_CUDA(cudaMemcpy(cid.data(), A->ell_class, cid.size(), cudaMemcpyDeviceToHost));
+        VEXB_CUDA(cudaMemcpy(ctab.data(), A->ell_ctab, ctab.size(), cudaMemcpyDeviceToHost));
+    }
+    if (ell_col && ne && (A->ell_mask || A->ell_class)) {
         // slot masks: column of slot k = row + shift of slot k where the row's mask has bit k, else -1
         std::vector<EllDiag> mask(A->ell_pitch);
-        VEXB_CUDA(cudaMemcpy(mask.data(), A->ell_mask, A->ell_pitch * sizeof(EllDiag), cudaMemcpyDeviceToHost));
+        if (A->ell_mask) VEXB_CUDA(cudaMemcpy(mask.data(), A->ell_mask, A->ell_pitch * sizeof(EllDiag), cudaMemcpyDeviceToHost));
+        else for (size_t i = 0; i < A->ell_pitch; ++i) mask[i].mask = ctab[cid[i]];
         for (size_t k = 0; k < A->ell_width; ++k)
             for (size_t i = 0; i < A->ell_pitch; ++i)
                 ell_col[i + A->ell_pitch * k] = (mask[i].mask >> k) & 1u ? (int32_t)((long long)i + A->ell_shifts.s[k]) : -1;
@@ -1552,7 +1672,11 @@ extern "C" int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, v
                 ell_col[i + A->ell_pitch * k] = raw == (short)-32768 ? -1 : (int32_t)((long long)i + A->ell_shifts.s[std::min<size_t>(k, vexb::kEllShiftSlots - 1)] + raw);
             }
     }
-    if (ell_val && ne) VEXB_CUDA(cudaMemcpy(ell_val, A->ell_val, ne * vs, cudaMemcpyDeviceToHost));
+    if (ell_val && ne && A->ell_class) {
+        for (size_t k = 0; k < A->ell_width; ++k)
+            for (size_t i = 0; i < A->ell_pitch; ++i)
+                memcpy((char *)ell_val + (i + A->ell_pitch * k) * vs, &ctab[kEllClassHeader + ((size_t)cid[i] * A->ell_width + k) * vs], vs);
+    } else if (ell_val && ne) VEXB_CUDA(cudaMemcpy(ell_val, A->ell_val, ne * vs, cudaMemcpyDeviceToHost));
     if (ell_col && ell_val && ne) {
         // the reference's packing: a row's entries in slots 0, 1, ... (the device layout may leave gaps, see build())
         for (size_t i = 0; i < A->nrows_stored; ++i) {

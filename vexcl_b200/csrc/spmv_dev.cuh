@@ -72,6 +72,57 @@ __device__ __forceinline__ double ldg_stream(const double *p, uint64_t policy) {
 __device__ __forceinline__ float ldg_stream(const float *p, uint64_t policy) {
     float v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(policy)); return v;
 }
+__device__ __forceinline__ unsigned ldg_stream(const EllClass *p, uint64_t policy) {
+    unsigned v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(policy)); return v;
+}
+// Class-table lookups (L1-resident, a broadcast when a warp's rows share a class).  volatile like the gathers of x, so
+// the compiler keeps them after those: a lookup waits for the row's class byte, and the gathers must not wait with it.
+__device__ __forceinline__ unsigned ldg_table(const unsigned char *p) {
+    unsigned v; asm volatile("ld.global.nc.u8 %0, [%1];" : "=r"(v) : "l"(p)); return v;
+}
+__device__ __forceinline__ double ldg_table(const double *p) {
+    double v; asm volatile("ld.global.nc.f64 %0, [%1];" : "=d"(v) : "l"(p)); return v;
+}
+__device__ __forceinline__ float ldg_table(const float *p) {
+    float v; asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p)); return v;
+}
+
+// Column that slot j of a row-class strip gathers whether or not the row's slot holds an entry: row + shift of slot j,
+// clamped to the strip's largest column x_max (a negative column wraps around to a large unsigned one), so that
+// a padding slot still reads inside x.
+__device__ __forceinline__ unsigned ell_class_column(size_t row, const EllShifts &sh, int j) {
+    return min((unsigned)((int)row + sh.s[j]), (unsigned)sh.x_max);
+}
+
+// R rows of a row-class strip (spmv.ell_classes), sum[r] for row i[r].  All R class bytes and all R*W gathers of x are
+// issued before the first table lookup: the column of slot k is row + shift of slot k whatever the row's mask says, so
+// the gathers need not wait for the class byte.  A gather whose slot is padding reads x at a clamped address (ell_class_column)
+// and is never added.  The set slots are added in slot order with the stored values, then
+// the CSR tail: the same bits as the other encodings.
+template <class T, int W, int R>
+__device__ __forceinline__ void hell_class_rows(const size_t (&i)[R], const EllClass *__restrict__ cls, const EllShifts &sh,
+                                                const T *__restrict__ table, const int *__restrict__ tail_ptr,
+                                                const int *__restrict__ tail_col, const T *__restrict__ tail_val,
+                                                const T *__restrict__ x, uint64_t stream, uint64_t keep, T (&sum)[R]) {
+    static_assert(W > 0 && W <= (int)kEllDiagMaxWidth, "row classes hold one slot mask byte: unrolled widths up to 8 only");
+    unsigned id[R]; T xv[R][W];
+#pragma unroll
+    for (int r = 0; r < R; ++r) id[r] = ldg_stream(cls + i[r], stream);
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+#pragma unroll
+        for (int j = 0; j < W; ++j) xv[r][j] = ldg_keep(x + ell_class_column(i[r], sh, j), keep);
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const unsigned m = ldg_table(reinterpret_cast<const unsigned char *>(table) + id[r]);
+        const T *v = table + kEllClassHeader / sizeof(T) + id[r] * W;
+        sum[r] = T(0);
+#pragma unroll
+        for (int j = 0; j < W; ++j) if ((m >> j) & 1u) sum[r] = t_add<T>(sum[r], t_mul<T>(ldg_table(v + j), xv[r][j]));
+        if (tail_ptr)
+            for (int j = tail_ptr[i[r]], e = tail_ptr[i[r] + 1]; j < e; ++j) sum[r] = t_add<T>(sum[r], t_mul<T>(tail_val[j], __ldg(x + tail_col[j])));
+    }
+}
 
 template <class T>
 __device__ __forceinline__ void store_y(T *y, size_t r, T sum, T alpha, int append) {
@@ -80,35 +131,43 @@ __device__ __forceinline__ void store_y(T *y, size_t r, T sum, T alpha, int appe
 }
 
 // One row of a hybrid-ELL strip (hybrid_ell.inl:252-268): ELL slots in order, then the CSR tail; products and sums rounded
-// separately.  W > 0: fully unrolled, all 2W streaming loads and then the W gathers of x in flight at once.
+// separately.  W > 0: fully unrolled, all 2W streaming loads and then the W gathers of x in flight at once.  Row-class
+// strips: hell_class_rows for one row.
 template <class T, int W, class C>
 __device__ __forceinline__ T hell_row_sum(size_t i, size_t pitch, int w_dyn, const C *__restrict__ ell_col, const EllShifts &shift,
                                           const T *__restrict__ ell_val, const int *__restrict__ tail_ptr,
                                           const int *__restrict__ tail_col, const T *__restrict__ tail_val,
                                           const T *__restrict__ x, uint64_t stream, uint64_t keep) {
     static_assert(W > 0 || !std::is_same<C, EllDiag>::value, "the diagonal encoding needs one shift per slot: unrolled widths only");
-    T sum = T(0);
-    const unsigned mask = ell_row_mask(ell_col, i, stream);
-    if (W > 0) {
-        int c[W > 0 ? W : 1]; T v[W > 0 ? W : 1]; T xv[W > 0 ? W : 1];
-#pragma unroll
-        for (int j = 0; j < W; ++j) { c[j] = ell_slot_column(ell_col, i, pitch, j, ell_shift_of(shift, j), mask, stream); v[j] = ldg_stream(ell_val + i + (size_t)j * pitch, stream); }
-#pragma unroll
-        for (int j = 0; j < W; ++j) xv[j] = (c[j] != -1) ? ldg_keep(x + c[j], keep) : T(0);
-#pragma unroll
-        for (int j = 0; j < W; ++j) if (c[j] != -1) sum = t_add<T>(sum, t_mul<T>(v[j], xv[j]));
+    if constexpr (std::is_same<C, EllClass>::value) {
+        const size_t rows[1] = {i};
+        T s[1];
+        hell_class_rows<T, W, 1>(rows, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep, s);
+        return s[0];
     } else {
-        // any width: plain dependent loop rather than batches of 4 columns: occupancy hides the latency, and a
-        // padded slot (column -1) costs 4 bytes, not 12, because its value is never fetched.
-        for (int j = 0; j < w_dyn; ++j) {
-            const int c = ell_slot_column(ell_col, i, pitch, j, shift.s[0], mask, stream);   // run-time widths use one shift (spmv.cu build())
-            if (c != -1) sum = t_add<T>(sum, t_mul<T>(ldg_stream(ell_val + i + (size_t)j * pitch, stream), ldg_keep(x + c, keep)));
+        T sum = T(0);
+        const unsigned mask = ell_row_mask(ell_col, i, stream);
+        if (W > 0) {
+            int c[W > 0 ? W : 1]; T v[W > 0 ? W : 1]; T xv[W > 0 ? W : 1];
+#pragma unroll
+            for (int j = 0; j < W; ++j) { c[j] = ell_slot_column(ell_col, i, pitch, j, ell_shift_of(shift, j), mask, stream); v[j] = ldg_stream(ell_val + i + (size_t)j * pitch, stream); }
+#pragma unroll
+            for (int j = 0; j < W; ++j) xv[j] = (c[j] != -1) ? ldg_keep(x + c[j], keep) : T(0);
+#pragma unroll
+            for (int j = 0; j < W; ++j) if (c[j] != -1) sum = t_add<T>(sum, t_mul<T>(v[j], xv[j]));
+        } else {
+            // any width: plain dependent loop rather than batches of 4 columns: occupancy hides the latency, and a
+            // padded slot (column -1) costs 4 bytes, not 12, because its value is never fetched.
+            for (int j = 0; j < w_dyn; ++j) {
+                const int c = ell_slot_column(ell_col, i, pitch, j, shift.s[0], mask, stream);   // run-time widths use one shift (spmv.cu build())
+                if (c != -1) sum = t_add<T>(sum, t_mul<T>(ldg_stream(ell_val + i + (size_t)j * pitch, stream), ldg_keep(x + c, keep)));
+            }
         }
+        if (tail_ptr) {
+            for (int j = tail_ptr[i], e = tail_ptr[i + 1]; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(tail_val[j], __ldg(x + tail_col[j])));
+        }
+        return sum;
     }
-    if (tail_ptr) {
-        for (int j = tail_ptr[i], e = tail_ptr[i + 1]; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(tail_val[j], __ldg(x + tail_col[j])));
-    }
-    return sum;
 }
 
 } // namespace vexb
