@@ -2,9 +2,11 @@
 """A/B of row classes against slot masks for hybrid-ELL strips in one process: spmv.ell_classes = 1 (the default; 2
 below the L2-size floor) against spmv.ell_classes = 0.
 
-    python scripts/ell_class_probe.py [--reps 200] [--rounds 5] > out.json
+    python scripts/ell_class_probe.py [--reps 200] [--rounds 5] [--copy-only] > out.json
 
-Times, with CUDA events over `reps` back-to-back launches and the two encodings alternating `rounds` times:
+First times A.apply on configs[2] against a copy y = x of the same two vectors, alternating (key "copy of the same x
+and y"): the copy moves the 16 bytes of x and y per row that the product cannot avoid, so it is the product's ceiling.
+Then times, with CUDA events over `reps` back-to-back launches and the two encodings alternating `rounds` times:
 A.apply on configs[2] (2-D 5-point, 3162^2) and configs[3] (3-D 7-point, 256^3), SpMat * multivector<4> on configs[2],
 one fused CG iteration (product + dot, two sweeps; CUDA graphs) on the 256^3 SPD Laplacian, and A.apply on a 2-D
 5-point strip of 1000^2 rows, whose 40 MB of values fit the 50 MB L2 (the size floor).  The results of the two
@@ -24,6 +26,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 import vexcl_b200 as vx                                    # noqa: E402
 from vexcl_b200 import gen                                 # noqa: E402
+from vexcl_b200 import _lib as L                           # noqa: E402
 from vexcl_b200.api import Event                           # noqa: E402
 
 
@@ -94,13 +97,46 @@ def products(ctx, key, dim, nx, reps, rounds, out, on=1, multi=False):
         out[key + " SpMat * multivector<4>"] = res
 
 
+def copy_ceiling(ctx, reps, rounds, out):
+    """A.apply on configs[2] against y = x on the same two vectors, which moves the same x and y bytes: the ceiling of
+    a kernel with this 1:1 read/write mix.  The copy runs both as the generated elementwise kernel (y.assign(x)) and
+    as cudaMemcpyAsync device to device."""
+    row, col, val = gen.poisson_strip(2, 3162)
+    n = row.size - 1
+    A = vx.SpMat(ctx, n, n, row, col, val)
+    del row, col, val
+    assert A.info().loc.ell_classes > 0
+    x, y = vx.vector(ctx, n), vx.vector(ctx, n)
+    x.assign(vx.ElementIndex() * (1.0 / n) + 0.25)
+    k = ctx.local[0]
+    fns = {"apply": lambda: A.apply(x, y), "copy": lambda: y.assign(x),
+           "memcpy": lambda: L.check(L.lib().vexb_d2d(ctx.devs[k], y.bufs[k], x.bufs[k], 8 * n, ctx.streams[k]))}
+    t = {f: [] for f in fns}
+    for _ in range(rounds):
+        for f, fn in fns.items():
+            t[f].append(timed(ctx, fn, reps))
+    med = {f: statistics.median(v) for f, v in t.items()}
+    out["copy of the same x and y"] = {
+        "rows": n, "ms_apply": med["apply"], "ms_copy": med["copy"], "ms_memcpy": med["memcpy"],
+        "apply_over_copy": med["apply"] / med["copy"], "apply_over_memcpy": med["apply"] / med["memcpy"],
+        "copy_TBps": 16 * n / (med["copy"] * 1e-3) / 1e12, "memcpy_TBps": 16 * n / (med["memcpy"] * 1e-3) / 1e12,
+        "apply_TBps_of_x_and_y": 16 * n / (med["apply"] * 1e-3) / 1e12,
+        "all_ms_apply": t["apply"], "all_ms_copy": t["copy"], "all_ms_memcpy": t["memcpy"]}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--copy-only", action="store_true", help="time only A.apply on configs[2] against the copy y = x")
     args = ap.parse_args()
     ctx = vx.Context([0])
     out = {"card": card(), "reps": args.reps, "rounds": args.rounds}
+
+    copy_ceiling(ctx, args.reps, args.rounds, out)
+    if args.copy_only:
+        print(json.dumps(out))
+        return
 
     products(ctx, "configs[2] 2-D 5-pt 3162^2", 2, 3162, args.reps, args.rounds, out, multi=True)
     products(ctx, "configs[3] 3-D 7-pt 256^3", 3, 256, args.reps, args.rounds, out)

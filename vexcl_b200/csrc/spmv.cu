@@ -474,21 +474,40 @@ __global__ void __launch_bounds__(kPipeThreads) csr_pipe_kernel(const int2 *__re
 // Rows per thread of hell_kernel on row-class strips.  Measured on configs[2] / configs[3] (H100 80GB HBM3, 400 W):
 // 1 row 0.080 / 0.137 ms, 2 rows 0.077 / 0.126 ms, 4 rows 0.083 / 0.140 ms.
 constexpr int kEllClassRows = 2;
+// How many blocks ahead hell_kernel prefetches into L2 on row-class strips.  Measured on configs[2] / configs[3]
+// (H100 80GB HBM3, 700 W), ms per product: none 0.0776 / 0.126, 132 0.0695 / 0.117, 264 and 528 0.0693 / 0.117,
+// 792 0.0695 / 0.117, 1584 0.0703 / 0.118, 3168 0.0912 / 0.152 (prefetched lines evicted before their rows run).
+// In bench.py (400 W card) 132 blocks cost configs[3] less than 528 (+1.4 % against +3.9 %) for the same gain on configs[2].
+constexpr int kEllClassPrefetchBlocks = 132;
 
 template <class T, int W, class C>
 __global__ void __launch_bounds__(256) hell_kernel(size_t n, size_t pitch, int w_dyn, const C *__restrict__ ell_col, const EllShifts shift,
                                                     const T *__restrict__ ell_val, const int *__restrict__ tail_ptr,
                                                     const int *__restrict__ tail_col, const T *__restrict__ tail_val,
                                                     const T *__restrict__ x, T *y, T alpha, int append,
-                                                    const int *__restrict__ row_ids) {
+                                                    const int *__restrict__ row_ids, int prefetch_blocks) {
     if constexpr (std::is_same<C, EllClass>::value) {
         // Row classes: a row moves 17 bytes (class, x, y), too few for one row per thread to keep enough bytes in flight.
         // A thread takes kEllClassRows rows, a block apart, so at every sub-step a warp's lanes hold consecutive rows
         // (coalesced class bytes and y stores); rows past the end repeat row n-1 and store nothing.
         constexpr int R = kEllClassRows;
+        const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+        if (threadIdx.x == 0 && prefetch_blocks > 0) {
+            // The rows of the block prefetch_blocks ahead: their class bytes and the x window of the largest shift, the
+            // first touch of its lines (the other slots read them again later, from L2).  HBM then streams while this
+            // block's threads wait on their own loads.
+            const long long f0 = ((long long)blockIdx.x + prefetch_blocks) * blockDim.x * R;
+            if (f0 < (long long)n) {
+                const long long f1 = min(f0 + (long long)blockDim.x * R, (long long)n);
+                int dmax = shift.s[0];
+#pragma unroll
+                for (int j = 1; j < W; ++j) dmax = max(dmax, shift.s[j]);
+                prefetch_l2(x, f0 + dmax, f1 + dmax, (long long)shift.x_max + 1, keep);
+                prefetch_l2(ell_col, f0, f1, (long long)n, stream);
+            }
+        }
         const size_t i0 = (size_t)blockIdx.x * blockDim.x * R + threadIdx.x;
         if (i0 >= n) return;
-        const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
         size_t rows[R]; T sum[R];
 #pragma unroll
         for (int r = 0; r < R; ++r) rows[r] = min(i0 + (size_t)r * blockDim.x, n - 1);
@@ -497,6 +516,7 @@ __global__ void __launch_bounds__(256) hell_kernel(size_t n, size_t pitch, int w
         for (int r = 0; r < R; ++r)
             if (i0 + (size_t)r * blockDim.x < n) store_y<T>(y, row_ids ? (size_t)row_ids[rows[r]] : rows[r], sum[r], alpha, append);
     } else {
+        (void)prefetch_blocks;
         const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
         if (i >= n) return;
         const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
@@ -1428,14 +1448,14 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
         const unsigned blocks = (unsigned)((n + 255) / 256);
 #define HL(W) do { \
             if (A->ell_col16) hell_kernel<T, W, short><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col16, A->ell_shifts, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids); \
+                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0); \
             else hell_kernel<T, W, int><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col, EllShifts{}, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids); } while (0)
+                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0); } while (0)
 #define HD(W) hell_kernel<T, W, EllDiag><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_mask, A->ell_shifts, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids)
+                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0)
 #define HC(W) hell_kernel<T, W, EllClass><<<(unsigned)((n + 256 * kEllClassRows - 1) / (256 * kEllClassRows)), 256, 0, st>>>( \
                   n, A->ell_pitch, (int)A->ell_width, A->ell_class, A->ell_shifts, (const T *)A->ell_ctab, A->tail_ptr, A->tail_col, \
-                  (const T *)A->tail_val, x, y, alpha, append, A->row_ids)
+                  (const T *)A->tail_val, x, y, alpha, append, A->row_ids, kEllClassPrefetchBlocks)
         if (A->ell_class) {
             switch (A->ell_width) {   // = the widths build() gives row classes: those of slot masks
                 case 3: HC(3); break; case 5: HC(5); break; case 7: HC(7); break;

@@ -31,6 +31,18 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src, uint32
                  :: "r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
 }
 
+// Asks L2 to fetch the 16-byte-aligned part of p[lo, hi), clipped to p[0, end).  A hint: no data comes back, no
+// register waits for it, and nothing outside p[0, end) is touched.
+template <class E>
+__device__ __forceinline__ void prefetch_l2(const E *p, long long lo, long long hi, long long end, uint64_t policy) {
+    lo = max(lo, 0ll); hi = min(hi, end);
+    if (hi <= lo) return;
+    const uintptr_t a = ((uintptr_t)(p + lo) + 15) & ~(uintptr_t)15, b = (uintptr_t)(p + hi) & ~(uintptr_t)15;
+    if (b > a)
+        asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;"
+                     :: "l"(a), "r"((uint32_t)(b - a)), "l"(policy) : "memory");
+}
+
 __device__ __forceinline__ double ldg_keep(const double *p, uint64_t policy) {
     double v; asm volatile("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(policy)); return v;
 }
