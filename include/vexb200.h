@@ -21,6 +21,10 @@
  *   vexb_csr_create /
  *   vexb_spmv           <- SpMatCSR / SpMatHELL ctor + mul_local/mul_remote
  *                          (vexcl/spmat/csr.inl:45-209, hybrid_ell.inl:53-330)
+ *   vexb_bsr_create /
+ *   vexb_bspmv          <- sparse::matrix<block value> ctor + product with the
+ *                          value types of rhs_of / spmv_ops_impl
+ *                          (vexcl/sparse/distributed.hpp:17-21, spmv_ops.hpp)
  *   vexb_dspmat_*       <- SpMat ctor + SpMat::apply (vexcl/spmat.hpp:71-185)
  *   vexb_ccsr_*         <- SpMatCCSR ctor + its generated product function
  *                          (vexcl/spmat/ccsr.hpp:70-78, :176-201)
@@ -429,6 +433,35 @@ int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, void *ell_va
                              int64_t *csr_ptr, int32_t *csr_col, void *csr_val);
 /* y (=|+=) alpha * A x     (csr.inl:188-209: append ? "+=" : "=") */
 int vexb_spmv(int dev, void *stream, const vexb_spmat *A, const void *x, void *y, double alpha, int append);
+
+/* ------------------------------------------------------------------------
+ * Block sparse strips (one device): B x B blocks as values, B = 2, 3 or 4 --
+ * vex::sparse::{csr, ell, matrix}<std::array<std::array<T,B>,B>>, the
+ * reference's custom value types (sparse/distributed.hpp:17-21 rhs_of,
+ * tests/sparse_matrices.cpp:239-282).  Stored as sliced ELL over block rows
+ * (the layout of VEXB_FMT_SELL, "spmv.sell_sigma"), one 32-bit block column
+ * per slot and the B*B values of a slot planar, so that a warp's value loads
+ * are 32 consecutive elements.
+ *   y_i (=|+=) alpha * sum over the blocks j of block row i, in storage order,
+ *   of A_j x_col(j); row r of a block is t = a_r0 x_0 + a_r1 x_1 + ... added
+ *   left to right, then s_r = s_r + t, every product and sum rounded on its own.
+ * create() validates every argument before it touches a device.
+ * ---------------------------------------------------------------------- */
+typedef struct vexb_bspmat vexb_bspmat;
+typedef struct {
+    size_t  nrows, ncols, nnzb;      /* block rows, block columns, stored blocks */
+    int32_t block, val_dtype;        /* B; VEXB_F64 or VEXB_F32 */
+    size_t  n_slices, n_slots;       /* sliced-ELL slices of 32 block rows, slots over all slices (as vexb_csr_sell_layout) */
+    size_t  device_bytes;            /* n_slots * (B*B*sizeof(T) + 4) + perm + slice_ptr */
+} vexb_bspmat_info;
+/* nrows/ncols/ptr/col count BLOCK rows/columns; val: nnzb blocks of B*B values, row-major inside a block;
+ * x: ncols*B values, y: nrows*B values (block i = elements [i*B, i*B+B)). */
+int vexb_bsr_create(int dev, void *stream, size_t nrows, size_t ncols, int block, const void *ptr, int ptr_bytes,
+                    const void *col, int col_bytes, const void *val, int val_dtype, vexb_bspmat **out);
+int vexb_bspmat_destroy(vexb_bspmat *A);
+int vexb_bspmat_get_info(const vexb_bspmat *A, vexb_bspmat_info *info);
+/* y (=|+=) alpha * A x; with no stored block, y = A*x zeroes y and y += A*x leaves it as it is (as vexb_spmv). */
+int vexb_bspmv(int dev, void *stream, const vexb_bspmat *A, const void *x, void *y, double alpha, int append);
 
 /* ------------------------------------------------------------------------
  * Compressed CSR for stencil-like matrices: vex::SpMatCCSR

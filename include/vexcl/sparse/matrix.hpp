@@ -6,7 +6,9 @@
  * csr -> the TMA-staged CSR row-block kernel, ell -> hybrid ELL (the reference's layout and width
  * rule; its device-side csr2ell conversion, ell.hpp:348-506, happens on the host at upload here),
  * matrix -> libvexb200's own choice (the reference picks csr on CPUs and ell on GPUs).
+ * With B x B block values (std::array<std::array<T, B>, B>) all three are the block format below.
  */
+#include <array>
 #include <iterator>
 #include <memory>
 #include "../vector.hpp"
@@ -66,6 +68,74 @@ class single_device_matrix {
         std::vector<backend::command_queue> q;
         size_t n, m, nnz;
         std::shared_ptr<vexb_spmat> A;
+};
+
+/// Value type of a vector multiplied by a matrix with value type V (vexcl/sparse/distributed.hpp:17-21): V itself, and
+/// std::array<T, B> for B x B blocks.
+template <class V, class Enable = void> struct rhs_of { typedef V type; };
+template <class T, size_t B> struct rhs_of<std::array<std::array<T, B>, B>> { typedef std::array<T, B> type; };
+
+namespace detail_sparse {
+template <class V> struct is_block_value : std::false_type {};
+template <class T, size_t B> struct is_block_value<std::array<std::array<T, B>, B>> : std::true_type {};
+}
+
+/// Block matrices: B x B blocks of double or float as values (B = 2, 3, 4), the reference's custom value types
+/// (tests/sparse_matrices.cpp:239-282) for real blocks.  Row and column counts, ptr and col are in blocks; x and y are
+/// vex::vector<std::array<T, B>>.  csr, ell and matrix all take the one block format of libvexb200 (sliced ELL over
+/// block rows, vexb_bsr_create).  `Y = A * X`, `Y += A * X` and `Y -= A * X` are one vexb_bspmv launch into Y; the
+/// product has no kernel form, so it takes part in no other expression.
+template <int Format, typename T, size_t B, typename Col, typename Ptr>
+class single_device_matrix<Format, std::array<std::array<T, B>, B>, Col, Ptr> {
+    public:
+        typedef std::array<std::array<T, B>, B> value_type; typedef value_type val_type; typedef Col col_type; typedef Ptr ptr_type;
+        typedef typename rhs_of<value_type>::type rhs_type;
+        static_assert(std::is_same<T, double>::value || std::is_same<T, float>::value, "block values must be double or float");
+        static_assert(B >= 2 && B <= 4, "blocks must be 2x2, 3x3 or 4x4");
+        static_assert(sizeof(rhs_type) == B * sizeof(T) && sizeof(value_type) == B * B * sizeof(T),
+                      "std::array must hold its elements without padding");
+
+        template <class PtrRange, class ColRange, class ValRange>
+        single_device_matrix(const std::vector<backend::command_queue> &q, size_t nrows, size_t ncols,
+                             const PtrRange &ptr, const ColRange &col, const ValRange &val, bool /*fast_setup*/ = true)
+            : q(q), n(nrows), m(ncols), nnz(detail_sparse::range_size(val))
+        {
+            precondition(q.size() == 1, "sparse matrices of this kind are only supported for single-device contexts");
+            static_assert(sizeof(Col) == 4 || sizeof(Col) == 8, "column type must be 32 or 64 bit");
+            static_assert(sizeof(Ptr) == 4 || sizeof(Ptr) == 8, "pointer type must be 32 or 64 bit");
+            vexb_bspmat *h = nullptr;
+            VEXB_CHECKED(vexb_bsr_create(q[0].ordinal(), q[0].raw(), nrows, ncols, static_cast<int>(B), detail_sparse::range_data(ptr),
+                                         sizeof(Ptr), detail_sparse::range_data(col), sizeof(Col), detail_sparse::range_data(val),
+                                         dtype_of<T>::value, &h));
+            A.reset(h, [](vexb_bspmat *p) { vexb_bspmat_destroy(p); });
+        }
+        single_device_matrix() : n(0), m(0), nnz(0) {}
+
+        size_t rows() const { return n; }
+        size_t cols() const { return m; }
+        size_t nonzeros() const { return nnz; }
+        const std::vector<backend::command_queue>& queue_list() const { return q; }
+
+        /// y = alpha * A * x   or   y += alpha * A * x
+        void mul(const vex::vector<rhs_type> &x, vex::vector<rhs_type> &y, double alpha = 1, bool append = false) const {
+            precondition(x.size() == m && y.size() == n, "sparse product: vector sizes do not match the matrix");
+            VEXB_CHECKED(vexb_bspmv(q[0].ordinal(), q[0].raw(), A.get(), x(0).raw(), y(0).raw(), alpha, append));
+        }
+
+        friend direct_product<single_device_matrix, vex::vector<rhs_type>> operator*(const single_device_matrix &A, const vex::vector<rhs_type> &x) {
+            return direct_product<single_device_matrix, vex::vector<rhs_type>>(A, x);
+        }
+        template <class Expr>
+        friend typename std::enable_if<is_vector_expr<Expr>::value && !std::is_same<Expr, vex::vector<rhs_type>>::value,
+                                       direct_product<single_device_matrix, Expr>>::type
+        operator*(const single_device_matrix &A, const Expr &x) {
+            static_assert(sizeof(Expr) == 0, "a block matrix multiplies a vex::vector<std::array<T, B>> of its own T and B only");
+            return direct_product<single_device_matrix, Expr>(A, x);
+        }
+    private:
+        std::vector<backend::command_queue> q;
+        size_t n, m, nnz;
+        std::shared_ptr<vexb_bspmat> A;
 };
 
 template <typename Val, typename Col = int, typename Ptr = Col> using csr    = single_device_matrix<VEXB_FMT_CSR,  Val, Col, Ptr>;

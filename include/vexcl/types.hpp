@@ -2,6 +2,7 @@
 #define VEXCL_TYPES_HPP
 // Element types understood by the back end and their names (subset of vexcl/types.hpp:202-260:
 // scalars only -- OpenCL vector types are outside the hot path).
+#include <array>
 #include <cstdint>
 #include <string>
 #include <type_traits>
@@ -42,6 +43,17 @@ template <> struct dtype_of<short> { static const int value = VEXB_I32; static c
 template <> struct dtype_of<signed char>    { static const int value = VEXB_I32; static const char *name() { return "char"; } };
 template <> struct dtype_of<unsigned char>  { static const int value = VEXB_I32; static const char *name() { return "uchar"; } };
 template <> struct dtype_of<unsigned short> { static const int value = VEXB_I32; static const char *name() { return "ushort"; } };
+
+// std::array<T, B> is the element of block vectors, vex::vector<std::array<T, B>> (and std::array<std::array<T, B>, B> the
+// value of block sparse matrices, sparse/matrix.hpp).  Block products write them with one call of their own; no
+// expression kernel takes them, so naming their element type is the point where any other use fails to compile.
+template <class T, size_t N> struct dtype_of<std::array<T, N>> {
+    static_assert(sizeof(T) == 0, "vex::vector<std::array<T, B>> holds block vectors: the only expressions on them are "
+                                  "Y = A * X, Y += A * X and Y -= A * X with a block matrix vex::sparse::{csr, ell, matrix}"
+                                  "<std::array<std::array<T, B>, B>>");
+    static const int value = -1;
+    static const char *name() { return "block"; }
+};
 
 template <class T> inline std::string type_name() { return dtype_of<typename std::decay<T>::type>::name(); }
 

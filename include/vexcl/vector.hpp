@@ -201,6 +201,10 @@ class vector : public vector_expr_tag {
         template <class M> const vector& operator=(const additive_operator<M, vector> &a)  { a.apply(*this, T(1), false); return *this; }
         template <class M> const vector& operator+=(const additive_operator<M, vector> &a) { a.apply(*this, T(1), true);  return *this; }
         template <class M> const vector& operator-=(const additive_operator<M, vector> &a) { a.apply(*this, T(-1), true); return *this; }
+        // block sparse products (sparse/matrix.hpp): one launch straight into y
+        template <class M> const vector& operator=(const direct_product<M, vector> &p)  { p.A.mul(p.x, *this, 1, false); return *this; }
+        template <class M> const vector& operator+=(const direct_product<M, vector> &p) { p.A.mul(p.x, *this, 1, true);  return *this; }
+        template <class M> const vector& operator-=(const direct_product<M, vector> &p) { p.A.mul(p.x, *this, -1, true); return *this; }
         const vector& operator=(const detail::additive_terms<T> &a)  { apply_terms(a, T(1), false); return *this; }
         const vector& operator+=(const detail::additive_terms<T> &a) { apply_terms(a, T(1), true);  return *this; }
         const vector& operator-=(const detail::additive_terms<T> &a) { apply_terms(a, T(-1), true); return *this; }

@@ -57,6 +57,11 @@ class SpmatInfo(C.Structure):
                 ("ell_classes", C.c_int32)]
 
 
+class BspmatInfo(C.Structure):
+    _fields_ = [("nrows", C.c_size_t), ("ncols", C.c_size_t), ("nnzb", C.c_size_t), ("block", C.c_int32),
+                ("val_dtype", C.c_int32), ("n_slices", C.c_size_t), ("n_slots", C.c_size_t), ("device_bytes", C.c_size_t)]
+
+
 class CcsrInfo(C.Structure):
     _fields_ = [("nrows", C.c_size_t), ("unique_rows", C.c_size_t), ("nnz", C.c_size_t), ("idx_bytes", C.c_int32),
                 ("table_in_smem", C.c_int32), ("device_bytes", C.c_size_t)]
@@ -152,6 +157,10 @@ def lib():
         "vexb_spmat_get_info": ([vp, P(SpmatInfo)], i),
         "vexb_spmat_hell_download": ([vp, vp, vp, vp, vp, vp], i),
         "vexb_spmv": ([i, vp, vp, vp, vp, d, i], i),
+        "vexb_bsr_create": ([i, vp, sz, sz, i, vp, i, vp, i, vp, i, P(vp)], i),
+        "vexb_bspmat_destroy": ([vp], i),
+        "vexb_bspmat_get_info": ([vp, P(BspmatInfo)], i),
+        "vexb_bspmv": ([i, vp, vp, vp, vp, d, i], i),
         "vexb_ccsr_create": ([i, vp, sz, sz, vp, i, vp, i, vp, i, vp, i, P(vp)], i),
         "vexb_ccsr_destroy": ([vp], i),
         "vexb_ccsr_get_info": ([vp, P(CcsrInfo)], i),

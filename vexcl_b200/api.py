@@ -1045,6 +1045,54 @@ class SpMatCCSR:
         return y
 
 
+class BlockMatrix:
+    """vex::sparse::matrix<std::array<std::array<T,B>,B>> (the reference's custom value types, sparse/distributed.hpp:17-21):
+    ptr/col count block rows and block columns, val has shape (nnzb, B, B), B = 2, 3 or 4.  x and y are plain vectors of
+    m*B and n*B scalars -- the bytes of vex::vector<std::array<T,B>>.  Single device."""
+
+    def __init__(self, ctx: Context, n: int, m: int, ptr, col, val):
+        if ctx.nparts != 1:
+            raise ValueError("block sparse matrices are only supported for single-device contexts")
+        self.ctx, self.n, self.m = ctx, int(n), int(m)
+        ptr, col, val = np.ascontiguousarray(ptr), np.ascontiguousarray(col), np.ascontiguousarray(val)
+        if ptr.dtype.itemsize not in (4, 8) or col.dtype.itemsize not in (4, 8):
+            raise TypeError("ptr/col must be 32- or 64-bit integers")
+        if val.ndim != 3 or val.shape[1] != val.shape[2]:
+            raise ValueError("val must have shape (nnzb, B, B)")
+        self.block = int(val.shape[1])
+        self.nnzb = int(val.shape[0])
+        self.val_dtype = _vdt(val.dtype)
+        self.h = C.c_void_p()
+        k = ctx.local[0]
+        L.check(L.lib().vexb_bsr_create(ctx.devs[k], ctx.streams[k], self.n, self.m, self.block, _ip(ptr), ptr.dtype.itemsize,
+                                        _ip(col), col.dtype.itemsize, _ip(val), self.val_dtype, C.byref(self.h)))
+
+    def __del__(self):
+        try:
+            L.lib().vexb_bspmat_destroy(self.h)
+        except Exception:
+            pass
+
+    def rows(self): return self.n
+    def cols(self): return self.m
+    def nonzeros(self): return self.nnzb
+
+    def info(self) -> L.BspmatInfo:
+        info = L.BspmatInfo()
+        L.check(L.lib().vexb_bspmat_get_info(self.h, C.byref(info)))
+        return info
+
+    def apply(self, x: vector, y: vector, alpha: float = 1.0, append: bool = False):
+        """y = alpha*A*x  or  y += alpha*A*x, one launch."""
+        if x.n != self.m * self.block or y.n != self.n * self.block:
+            raise ValueError("BlockMatrix::apply: vector sizes do not match the matrix")
+        if x.dtype != self.val_dtype or y.dtype != self.val_dtype:
+            raise TypeError("BlockMatrix::apply: vectors must have the matrix's value type")
+        k = self.ctx.local[0]
+        L.check(L.lib().vexb_bspmv(self.ctx.devs[k], self.ctx.streams[k], self.h, x.bufs[k], y.bufs[k], float(alpha), int(append)))
+        return y
+
+
 class stencil:
     """vex::stencil<T> (stencil.hpp:168-330): `y = x * s`, `y += x * s`, `y = 42 * (x * s)`, ...
     y[i] = sum_k s[k] * x[clamp(i + k - center)]; with several slices the neighbours' edge elements are copied
