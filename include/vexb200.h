@@ -25,6 +25,9 @@
  *   vexb_bspmv          <- sparse::matrix<block value> ctor + product with the
  *                          value types of rhs_of / spmv_ops_impl
  *                          (vexcl/sparse/distributed.hpp:17-21, spmv_ops.hpp)
+ *   vexb_zsr_create /
+ *   vexb_zspmv          <- sparse::matrix<std::complex<T>> ctor + product with
+ *                          the spmv_ops_impl of examples/complex_spmv.cpp
  *   vexb_dspmat_*       <- SpMat ctor + SpMat::apply (vexcl/spmat.hpp:71-185)
  *   vexb_ccsr_*         <- SpMatCCSR ctor + its generated product function
  *                          (vexcl/spmat/ccsr.hpp:70-78, :176-201)
@@ -462,6 +465,34 @@ int vexb_bspmat_destroy(vexb_bspmat *A);
 int vexb_bspmat_get_info(const vexb_bspmat *A, vexb_bspmat_info *info);
 /* y (=|+=) alpha * A x; with no stored block, y = A*x zeroes y and y += A*x leaves it as it is (as vexb_spmv). */
 int vexb_bspmv(int dev, void *stream, const vexb_bspmat *A, const void *x, void *y, double alpha, int append);
+
+/* ------------------------------------------------------------------------
+ * Complex sparse strips (one device): std::complex<T> values, T = double or
+ * float -- vex::sparse::{csr, ell, matrix}<std::complex<T>>, the reference's
+ * examples/complex_spmv.cpp (its spmv_ops_impl<std::complex<T>, ...>).
+ * Stored as the block strips above with 2 planar components (re, im) per slot
+ * instead of B*B.  For each stored entry a + bi of row i, in storage order:
+ *   s_re = s_re + (a xr - b xi),   s_im = s_im + (a xi + b xr),
+ * every product and sum rounded on its own; y_i (=|+=) alpha * s per
+ * component (alpha real).  The same bits as vexb_bspmv on the 2 x 2 blocks
+ * [[a, -b], [b, a]].  create() validates every argument before it touches a
+ * device.
+ * ---------------------------------------------------------------------- */
+typedef struct vexb_zspmat vexb_zspmat;
+typedef struct {
+    size_t  nrows, ncols, nnz;       /* rows, columns, stored complex entries */
+    int32_t val_dtype;               /* VEXB_F64 (complex<double>) or VEXB_F32 (complex<float>) */
+    size_t  n_slices, n_slots;       /* sliced-ELL slices of 32 rows, slots over all slices (as vexb_csr_sell_layout) */
+    size_t  device_bytes;            /* n_slots * (2*sizeof(T) + 4) + perm + slice_ptr */
+} vexb_zspmat_info;
+/* val: nnz interleaved (re, im) pairs of T, the bytes of std::complex<T>[nnz]; val_dtype names T.
+ * x: 2*ncols T and y: 2*nrows T, the bytes of std::complex<T>[]; x must be aligned to 2*sizeof(T). */
+int vexb_zsr_create(int dev, void *stream, size_t nrows, size_t ncols, const void *ptr, int ptr_bytes,
+                    const void *col, int col_bytes, const void *val, int val_dtype, vexb_zspmat **out);
+int vexb_zspmat_destroy(vexb_zspmat *A);
+int vexb_zspmat_get_info(const vexb_zspmat *A, vexb_zspmat_info *info);
+/* y (=|+=) alpha * A x, alpha real; with no stored entry, y = A*x zeroes y and y += A*x leaves it as it is. */
+int vexb_zspmv(int dev, void *stream, const vexb_zspmat *A, const void *x, void *y, double alpha, int append);
 
 /* ------------------------------------------------------------------------
  * Compressed CSR for stencil-like matrices: vex::SpMatCCSR

@@ -307,16 +307,16 @@ struct additive_operator {
     void apply(V &y, typename V::value_type sign, bool append) const { A.apply(x, y, sign * scale, append); }
 };
 
-/// `M * x` that M writes straight into y with one call, M::mul(x, y, alpha, append): the product of a block sparse matrix
-/// (sparse/matrix.hpp).  vex::vector takes it as y = A*x, y += A*x and y -= A*x.  It has no kernel form, so any other
+/// `M * x` that M writes straight into y with one call, M::mul(x, y, alpha, append): the product of a block or complex
+/// sparse matrix (sparse/matrix.hpp).  vex::vector takes it as y = A*x, y += A*x and y -= A*x.  It has no kernel form, so any other
 /// expression that holds it stops at the static_assert below.
 template <class M, class V>
 struct direct_product : vector_expr_tag {
     static const bool hold_by_reference = false;
-    typedef typename M::rhs_type::value_type value_type;   // the block's scalar: expression nodes around a misused product still form
+    typedef typename M::rhs_type::value_type value_type;   // the block's or complex's scalar: expression nodes around a misused product still form
     const M &A; const V &x;
     direct_product(const M &A, const V &x) : A(A), x(x) {}
-    void props(detail::expr_props&) const { static_assert(sizeof(M) == 0, "a block matrix product is only assigned: Y = A * X, Y += A * X or Y -= A * X"); }
+    void props(detail::expr_props&) const { static_assert(sizeof(M) == 0, "a block or complex matrix product is only assigned: Y = A * X, Y += A * X or Y -= A * X"); }
     int lower(detail::ir_builder&) const { return -1; }
 };
 

@@ -26,6 +26,8 @@ class distributed {
         typedef typename Matrix::ptr_type ptr_type;
         static_assert(!detail_sparse::is_block_value<value_type>::value,
                       "vex::sparse::distributed does not take block values: use vex::sparse::matrix on a single device");
+        static_assert(!detail_sparse::is_complex_value<value_type>::value,
+                      "vex::sparse::distributed does not take complex values: use vex::sparse::matrix on a single device");
 
         template <class PtrRange, class ColRange, class ValRange>
         distributed(const std::vector<backend::command_queue> &q, size_t nrows, size_t ncols,

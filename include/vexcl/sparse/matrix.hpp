@@ -6,9 +6,11 @@
  * csr -> the TMA-staged CSR row-block kernel, ell -> hybrid ELL (the reference's layout and width
  * rule; its device-side csr2ell conversion, ell.hpp:348-506, happens on the host at upload here),
  * matrix -> libvexb200's own choice (the reference picks csr on CPUs and ell on GPUs).
- * With B x B block values (std::array<std::array<T, B>, B>) all three are the block format below.
+ * With B x B block values (std::array<std::array<T, B>, B>) all three are the block format below, and with
+ * std::complex<T> values the complex format below.
  */
 #include <array>
+#include <complex>
 #include <iterator>
 #include <memory>
 #include "../vector.hpp"
@@ -138,7 +140,67 @@ class single_device_matrix<Format, std::array<std::array<T, B>, B>, Col, Ptr> {
         std::shared_ptr<vexb_bspmat> A;
 };
 
-template <typename Val, typename Col = int, typename Ptr = Col> using csr    = single_device_matrix<VEXB_FMT_CSR,  Val, Col, Ptr>;
+namespace detail_sparse {
+template <class V> struct is_complex_value : std::false_type {};
+template <class T> struct is_complex_value<std::complex<T>> : std::true_type {};
+}
+
+/// Complex matrices: std::complex<double> or std::complex<float> values, the reference's examples/complex_spmv.cpp.  x and
+/// y are vex::vector<std::complex<T>>.  csr, ell and matrix all take the one complex format of libvexb200 (sliced ELL,
+/// vexb_zsr_create).  `Y = A * X`, `Y += A * X` and `Y -= A * X` are one vexb_zspmv launch into Y; the product has no
+/// kernel form, so it takes part in no other expression.
+template <int Format, typename T, typename Col, typename Ptr>
+class single_device_matrix<Format, std::complex<T>, Col, Ptr> {
+    public:
+        typedef std::complex<T> value_type; typedef value_type val_type; typedef Col col_type; typedef Ptr ptr_type;
+        typedef typename rhs_of<value_type>::type rhs_type;
+        static_assert(std::is_same<T, double>::value || std::is_same<T, float>::value, "complex values must be std::complex<double> or std::complex<float>");
+        static_assert(sizeof(value_type) == 2 * sizeof(T), "std::complex must hold (re, im) without padding");
+
+        template <class PtrRange, class ColRange, class ValRange>
+        single_device_matrix(const std::vector<backend::command_queue> &q, size_t nrows, size_t ncols,
+                             const PtrRange &ptr, const ColRange &col, const ValRange &val, bool /*fast_setup*/ = true)
+            : q(q), n(nrows), m(ncols), nnz(detail_sparse::range_size(val))
+        {
+            precondition(q.size() == 1, "sparse matrices of this kind are only supported for single-device contexts");
+            static_assert(sizeof(Col) == 4 || sizeof(Col) == 8, "column type must be 32 or 64 bit");
+            static_assert(sizeof(Ptr) == 4 || sizeof(Ptr) == 8, "pointer type must be 32 or 64 bit");
+            vexb_zspmat *h = nullptr;
+            VEXB_CHECKED(vexb_zsr_create(q[0].ordinal(), q[0].raw(), nrows, ncols, detail_sparse::range_data(ptr), sizeof(Ptr),
+                                         detail_sparse::range_data(col), sizeof(Col), detail_sparse::range_data(val),
+                                         dtype_of<T>::value, &h));
+            A.reset(h, [](vexb_zspmat *p) { vexb_zspmat_destroy(p); });
+        }
+        single_device_matrix() : n(0), m(0), nnz(0) {}
+
+        size_t rows() const { return n; }
+        size_t cols() const { return m; }
+        size_t nonzeros() const { return nnz; }
+        const std::vector<backend::command_queue>& queue_list() const { return q; }
+
+        /// y = alpha * A * x   or   y += alpha * A * x, alpha real
+        void mul(const vex::vector<rhs_type> &x, vex::vector<rhs_type> &y, double alpha = 1, bool append = false) const {
+            precondition(x.size() == m && y.size() == n, "sparse product: vector sizes do not match the matrix");
+            VEXB_CHECKED(vexb_zspmv(q[0].ordinal(), q[0].raw(), A.get(), x(0).raw(), y(0).raw(), alpha, append));
+        }
+
+        friend direct_product<single_device_matrix, vex::vector<rhs_type>> operator*(const single_device_matrix &A, const vex::vector<rhs_type> &x) {
+            return direct_product<single_device_matrix, vex::vector<rhs_type>>(A, x);
+        }
+        template <class Expr>
+        friend typename std::enable_if<is_vector_expr<Expr>::value && !std::is_same<Expr, vex::vector<rhs_type>>::value,
+                                       direct_product<single_device_matrix, Expr>>::type
+        operator*(const single_device_matrix &A, const Expr &x) {
+            static_assert(sizeof(Expr) == 0, "a complex matrix multiplies a vex::vector<std::complex<T>> of its own T only");
+            return direct_product<single_device_matrix, Expr>(A, x);
+        }
+    private:
+        std::vector<backend::command_queue> q;
+        size_t n, m, nnz;
+        std::shared_ptr<vexb_zspmat> A;
+};
+
+template <typename Val, typename Col = int, typename Ptr = Col> using csr   = single_device_matrix<VEXB_FMT_CSR,  Val, Col, Ptr>;
 template <typename Val, typename Col = int, typename Ptr = Col> using ell    = single_device_matrix<VEXB_FMT_HELL, Val, Col, Ptr>;
 template <typename Val, typename Col = int, typename Ptr = Col> using matrix = single_device_matrix<VEXB_FMT_AUTO, Val, Col, Ptr>;
 

@@ -3,6 +3,7 @@
 // Element types understood by the back end and their names (subset of vexcl/types.hpp:202-260:
 // scalars only -- OpenCL vector types are outside the hot path).
 #include <array>
+#include <complex>
 #include <cstdint>
 #include <string>
 #include <type_traits>
@@ -53,6 +54,16 @@ template <class T, size_t N> struct dtype_of<std::array<T, N>> {
                                   "<std::array<std::array<T, B>, B>>");
     static const int value = -1;
     static const char *name() { return "block"; }
+};
+
+// std::complex<T> is the element of complex vectors, vex::vector<std::complex<T>>, and the value of complex sparse matrices
+// (sparse/matrix.hpp): as with blocks, only their products write them.
+template <class T> struct dtype_of<std::complex<T>> {
+    static_assert(sizeof(T) == 0, "vex::vector<std::complex<T>> holds complex vectors: the only expressions on them are "
+                                  "Y = A * X, Y += A * X and Y -= A * X with a complex matrix vex::sparse::{csr, ell, matrix}"
+                                  "<std::complex<T>>");
+    static const int value = -1;
+    static const char *name() { return "complex"; }
 };
 
 template <class T> inline std::string type_name() { return dtype_of<typename std::decay<T>::type>::name(); }

@@ -62,6 +62,11 @@ class BspmatInfo(C.Structure):
                 ("val_dtype", C.c_int32), ("n_slices", C.c_size_t), ("n_slots", C.c_size_t), ("device_bytes", C.c_size_t)]
 
 
+class ZspmatInfo(C.Structure):
+    _fields_ = [("nrows", C.c_size_t), ("ncols", C.c_size_t), ("nnz", C.c_size_t), ("val_dtype", C.c_int32),
+                ("n_slices", C.c_size_t), ("n_slots", C.c_size_t), ("device_bytes", C.c_size_t)]
+
+
 class CcsrInfo(C.Structure):
     _fields_ = [("nrows", C.c_size_t), ("unique_rows", C.c_size_t), ("nnz", C.c_size_t), ("idx_bytes", C.c_int32),
                 ("table_in_smem", C.c_int32), ("device_bytes", C.c_size_t)]
@@ -161,6 +166,10 @@ def lib():
         "vexb_bspmat_destroy": ([vp], i),
         "vexb_bspmat_get_info": ([vp, P(BspmatInfo)], i),
         "vexb_bspmv": ([i, vp, vp, vp, vp, d, i], i),
+        "vexb_zsr_create": ([i, vp, sz, sz, vp, i, vp, i, vp, i, P(vp)], i),
+        "vexb_zspmat_destroy": ([vp], i),
+        "vexb_zspmat_get_info": ([vp, P(ZspmatInfo)], i),
+        "vexb_zspmv": ([i, vp, vp, vp, vp, d, i], i),
         "vexb_ccsr_create": ([i, vp, sz, sz, vp, i, vp, i, vp, i, vp, i, P(vp)], i),
         "vexb_ccsr_destroy": ([vp], i),
         "vexb_ccsr_get_info": ([vp, P(CcsrInfo)], i),

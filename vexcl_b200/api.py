@@ -1093,6 +1093,53 @@ class BlockMatrix:
         return y
 
 
+class ComplexMatrix:
+    """vex::sparse::matrix<std::complex<T>> (the reference's examples/complex_spmv.cpp): val is complex128 or complex64.  x
+    and y are plain vectors of 2*m and 2*n scalars of the matching real type, the bytes of vex::vector<std::complex<T>>:
+    vector(ctx, z.view(np.float64)).  alpha is real.  Single device."""
+
+    def __init__(self, ctx: Context, n: int, m: int, ptr, col, val):
+        if ctx.nparts != 1:
+            raise ValueError("complex sparse matrices are only supported for single-device contexts")
+        self.ctx, self.n, self.m = ctx, int(n), int(m)
+        ptr, col, val = np.ascontiguousarray(ptr), np.ascontiguousarray(col), np.ascontiguousarray(val)
+        if ptr.dtype.itemsize not in (4, 8) or col.dtype.itemsize not in (4, 8):
+            raise TypeError("ptr/col must be 32- or 64-bit integers")
+        if val.dtype not in (np.complex128, np.complex64) or val.ndim != 1:
+            raise TypeError("val must be a 1-d complex128 or complex64 array")
+        self.nnz = int(val.size)
+        self.val_dtype = L.F64 if val.dtype == np.complex128 else L.F32
+        self.h = C.c_void_p()
+        k = ctx.local[0]
+        L.check(L.lib().vexb_zsr_create(ctx.devs[k], ctx.streams[k], self.n, self.m, _ip(ptr), ptr.dtype.itemsize,
+                                        _ip(col), col.dtype.itemsize, _ip(val), self.val_dtype, C.byref(self.h)))
+
+    def __del__(self):
+        try:
+            L.lib().vexb_zspmat_destroy(self.h)
+        except Exception:
+            pass
+
+    def rows(self): return self.n
+    def cols(self): return self.m
+    def nonzeros(self): return self.nnz
+
+    def info(self) -> L.ZspmatInfo:
+        info = L.ZspmatInfo()
+        L.check(L.lib().vexb_zspmat_get_info(self.h, C.byref(info)))
+        return info
+
+    def apply(self, x: vector, y: vector, alpha: float = 1.0, append: bool = False):
+        """y = alpha*A*x  or  y += alpha*A*x, one launch."""
+        if x.n != 2 * self.m or y.n != 2 * self.n:
+            raise ValueError("ComplexMatrix::apply: vector sizes do not match the matrix")
+        if x.dtype != self.val_dtype or y.dtype != self.val_dtype:
+            raise TypeError("ComplexMatrix::apply: vectors must have the real type of the matrix's values")
+        k = self.ctx.local[0]
+        L.check(L.lib().vexb_zspmv(self.ctx.devs[k], self.ctx.streams[k], self.h, x.bufs[k], y.bufs[k], float(alpha), int(append)))
+        return y
+
+
 class stencil:
     """vex::stencil<T> (stencil.hpp:168-330): `y = x * s`, `y += x * s`, `y = 42 * (x * s)`, ...
     y[i] = sum_k s[k] * x[clamp(i + k - center)]; with several slices the neighbours' edge elements are copied

@@ -1,21 +1,35 @@
-// Block sparse strips on one device: y (=|+=) alpha * A * x with B x B blocks (B = 2, 3, 4) as values, the product
-// of vex::sparse::{csr, ell, matrix}<std::array<std::array<T,B>,B>> (the reference's custom value types,
-// sparse/distributed.hpp:17-21 rhs_of + sparse/spmv_ops.hpp spmv_ops_impl).
+// Block and complex sparse strips on one device: y (=|+=) alpha * A * x with B x B blocks (B = 2, 3, 4) or complex numbers
+// as values, the products of vex::sparse::{csr, ell, matrix}<std::array<std::array<T,B>,B>> (the reference's custom value
+// types, sparse/distributed.hpp:17-21 rhs_of + sparse/spmv_ops.hpp spmv_ops_impl) and of vex::sparse::{csr, ell,
+// matrix}<std::complex<T>> (the spmv_ops_impl of the reference's examples/complex_spmv.cpp).
 //
 // Layout: sliced ELL (SELL-32-sigma, as VEXB_FMT_SELL) over BLOCK rows, from the same host sell_layout, sigma
 // ("spmv.sell_sigma") and perm / slice_ptr.  One int32 block column per slot (-1 = padding).  Values are planar per
 // slot: component c = r*B + q of slot k, lane l of slice s sits at val[(slice_ptr[s] + 32k) * B*B + 32c + l], so every
 // value load of a warp is 32 consecutive T whatever B is.  One column and one gather of B consecutive x values serve
 // B*B values: 8B^2 + 4 bytes per stored block in double against 12B^2 for the same block expanded into scalar CSR.
+// Complex strips are the same layout over rows with 2 components per slot, c = 0 (re) and c = 1 (im): 2 sizeof(T) + 4
+// bytes per stored entry, and one 2 sizeof(T)-byte gather of x (re, im) per slot.
 #include "hostlogic.hpp"
 #include "spmv_dev.cuh"
 #include <vector>
 
-struct vexb_bspmat {
-    int dev = 0, block = 0, val_dtype = VEXB_F64;
-    size_t nrows = 0, ncols = 0, nnzb = 0;     // block rows, block columns, stored blocks
+namespace vexb {
+// Device arrays of a sliced-ELL strip with planar values, shared by block and complex strips.
+struct sell_strip {
     int *slice_ptr = nullptr, *perm = nullptr, *col = nullptr; void *val = nullptr;
     size_t n_slices = 0, n_slots = 0, device_bytes = 0;
+};
+}
+
+struct vexb_bspmat : vexb::sell_strip {
+    int dev = 0, block = 0, val_dtype = VEXB_F64;
+    size_t nrows = 0, ncols = 0, nnzb = 0;     // block rows, block columns, stored blocks
+};
+
+struct vexb_zspmat : vexb::sell_strip {
+    int dev = 0, val_dtype = VEXB_F64;         // VEXB_F64: std::complex<double>, VEXB_F32: std::complex<float>
+    size_t nrows = 0, ncols = 0, nnz = 0;      // rows, columns, stored complex entries
 };
 
 namespace vexb {
@@ -97,6 +111,75 @@ static int bspmv_launch(const vexb_bspmat *A, cudaStream_t st, const T *x, T *y,
     return VEXB_OK;
 }
 
+template <class T> struct complex_of;
+template <> struct complex_of<double> { typedef double2 type; };
+template <> struct complex_of<float> { typedef float2 type; };
+
+// Slots in flight per loop turn: U * (2 values + 1 column) streaming loads and U gathers of x per lane.  No spills in
+// either precision (-Xptxas -v, DESIGN.md section 3 lists the register counts).
+constexpr int kZsellUnroll = 4;
+
+// The row's entries a + bi in storage order (the spmv_ops_impl of the reference's examples/complex_spmv.cpp):
+// s_re = s_re + (a xr - b xi), s_im = s_im + (a xi + b xr), every product and sum rounded on its own.
+template <class T, int U>
+__device__ __forceinline__ void zsell_slots(const int *cp, const T *vp, int k, const typename complex_of<T>::type *__restrict__ x,
+                                            uint64_t stream, uint64_t keep, T &re, T &im) {
+    typedef typename complex_of<T>::type C2;
+    int c[U]; T a[U], b[U]; C2 xv[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+        c[u] = ldg_stream(cp + (size_t)(k + u) * 32, stream);
+        a[u] = ldg_stream(vp + (size_t)(k + u) * 64, stream);
+        b[u] = ldg_stream(vp + (size_t)(k + u) * 64 + 32, stream);
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) xv[u] = c[u] != -1 ? ldg_keep(x + c[u], keep) : C2{T(0), T(0)};
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+        if (c[u] == -1) continue;
+        re = t_add<T>(re, t_sub<T>(t_mul<T>(a[u], xv[u].x), t_mul<T>(b[u], xv[u].y)));
+        im = t_add<T>(im, t_add<T>(t_mul<T>(a[u], xv[u].y), t_mul<T>(b[u], xv[u].x)));
+    }
+}
+
+// One warp per slice, one lane per row, the real and imaginary sums in registers.
+template <class T>
+__global__ void __launch_bounds__(256) zsell_kernel(size_t n_slices, const int *__restrict__ slice_ptr, const int *__restrict__ perm,
+                                                    const int *__restrict__ col, const T *__restrict__ val,
+                                                    const typename complex_of<T>::type *__restrict__ x, T *y, T alpha, int append) {
+    constexpr int U = kZsellUnroll;
+    const size_t s = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (s >= n_slices) return;
+    const int lane = threadIdx.x & 31;
+    const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+    const int base = __ldg(slice_ptr + s), w = (__ldg(slice_ptr + s + 1) - base) >> 5;
+    const int r = ldg_stream(perm + s * 32 + lane, stream);
+    const int *cp = col + base + lane;
+    const T *vp = val + (size_t)base * 2 + lane;
+    T re = T(0), im = T(0);
+    int k = 0;
+    for (; k + U <= w; k += U) zsell_slots<T, U>(cp, vp, k, x, stream, keep, re, im);
+    for (; k < w; ++k) zsell_slots<T, 1>(cp, vp, k, x, stream, keep, re, im);
+    if (r >= 0) {
+        store_y<T>(y, (size_t)r * 2, re, alpha, append);
+        store_y<T>(y, (size_t)r * 2 + 1, im, alpha, append);
+    }
+}
+
+template <class T>
+static int zspmv_launch(const vexb_zspmat *A, cudaStream_t st, const T *x, T *y, T alpha, int append) {
+    if (A->nrows == 0) return VEXB_OK;
+    if (A->nnz == 0) {
+        if (!append) VEXB_CUDA(cudaMemsetAsync(y, 0, A->nrows * 2 * sizeof(T), st));
+        return VEXB_OK;
+    }
+    const unsigned grid = (unsigned)((A->n_slices + 7) / 8);
+    zsell_kernel<T><<<grid, 256, 0, st>>>(A->n_slices, A->slice_ptr, A->perm, A->col, (const T *)A->val,
+                                          (const typename complex_of<T>::type *)x, y, alpha, append);
+    VEXB_LAUNCHED();
+    return VEXB_OK;
+}
+
 template <class E>
 static int upload_array(const std::vector<E> &h, void **d, size_t *bytes_acc) {
     *d = nullptr;
@@ -107,28 +190,74 @@ static int upload_array(const std::vector<E> &h, void **d, size_t *bytes_acc) {
     return VEXB_OK;
 }
 
-// Host packing of the planar slots (see the top of this file); padding slots keep column -1 and zero values.
+// Host form of a strip whose arguments passed sell_check: row pointers from 0, columns, and the sliced-ELL layout.
+struct sell_host {
+    std::vector<int> rp, col, perm, sptr;
+    size_t nnz = 0, slots = 0;
+};
+
+// The argument checks of vexb_bsr_create and vexb_zsr_create; none touches a device.  `unit` is "block " when rows,
+// columns and entries count blocks, "" otherwise.
+static int sell_check(size_t nrows, size_t ncols, const void *ptr, int ptr_bytes, const void *col, int col_bytes,
+                      const void *val, int val_dtype, const char *unit, sell_host &h) {
+    VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
+    VEXB_CHECK(ptr_bytes == 4 || ptr_bytes == 8, "ptr_bytes must be 4 or 8");
+    VEXB_CHECK(col_bytes == 4 || col_bytes == 8, "col_bytes must be 4 or 8");
+    VEXB_CHECK(nrows == 0 || ptr, "ptr is NULL");
+    VEXB_CHECK(nrows < (size_t)INT32_MAX && ncols < (size_t)INT32_MAX, "%sdimensions exceed 32-bit local indices", unit);
+    const int64_t p0 = nrows ? read_index(ptr, ptr_bytes, 0) : 0;
+    const int64_t nnz = nrows ? read_index(ptr, ptr_bytes, nrows) - p0 : 0;
+    VEXB_CHECK(nnz >= 0 && nnz < (int64_t)INT32_MAX - 64, "%lld stored %sentries do not fit 32-bit row pointers", (long long)nnz, unit);
+    VEXB_CHECK(nnz == 0 || (col && val), "col/val is NULL");
+    h.nnz = (size_t)nnz;
+    h.rp.assign(nrows + 1, 0);
+    h.col.resize((size_t)nnz);
+    for (size_t i = 1; i <= nrows; ++i) {
+        const int64_t v = read_index(ptr, ptr_bytes, i) - p0;
+        VEXB_CHECK(v >= h.rp[i - 1] && v <= nnz, "row pointers decrease at %srow %zu", unit, i);
+        h.rp[i] = (int)v;
+    }
+    for (size_t j = 0; j < (size_t)nnz; ++j) {
+        const int64_t cj = read_index(col, col_bytes, j);
+        VEXB_CHECK(cj >= 0 && (size_t)cj < ncols, "%scolumn %lld out of range at entry %zu", unit, (long long)cj, j);
+        h.col[j] = (int)cj;
+    }
+    VEXB_CHECK(sell_layout(nrows, h.rp.data(), param("spmv.sell_sigma", 1024), h.perm, h.sptr, &h.slots),
+               "%sstrip too large for 32-bit slot offsets", unit);
+    return VEXB_OK;
+}
+
+// Host packing of the planar slots (see the top of this file), `comps` values per stored entry; padding slots keep
+// column -1 and zero values.
 template <class T>
-static int bsr_upload(vexb_bspmat *A, const std::vector<int> &rp, const std::vector<int> &bcol, const T *val,
-                      const std::vector<int> &perm, const std::vector<int> &sptr) {
-    const size_t B = (size_t)A->block, BB = B * B;
-    std::vector<int> scol(A->n_slots, -1);
-    std::vector<T> sval(A->n_slots * BB, T(0));
-    for (size_t sl = 0; sl < A->n_slices; ++sl)
+static int sell_upload(sell_strip *S, const sell_host &h, const T *val, size_t comps) {
+    S->n_slices = h.sptr.size() - 1; S->n_slots = h.slots;
+    std::vector<int> scol(S->n_slots, -1);
+    std::vector<T> sval(S->n_slots * comps, T(0));
+    for (size_t sl = 0; sl < S->n_slices; ++sl)
         for (int l = 0; l < 32; ++l) {
-            const int r = perm[sl * 32 + l];
+            const int r = h.perm[sl * 32 + l];
             if (r < 0) continue;
-            for (int j = rp[r], k = 0; j < rp[r + 1]; ++j, ++k) {
-                const size_t slot = (size_t)sptr[sl] + (size_t)k * 32;
-                scol[slot + l] = bcol[j];
-                for (size_t c = 0; c < BB; ++c) sval[slot * BB + 32 * c + l] = val[(size_t)j * BB + c];
+            for (int j = h.rp[r], k = 0; j < h.rp[r + 1]; ++j, ++k) {
+                const size_t slot = (size_t)h.sptr[sl] + (size_t)k * 32;
+                scol[slot + l] = h.col[j];
+                for (size_t c = 0; c < comps; ++c) sval[slot * comps + 32 * c + l] = val[(size_t)j * comps + c];
             }
         }
-    VEXB_TRY(upload_array(sptr, (void **)&A->slice_ptr, &A->device_bytes));
-    VEXB_TRY(upload_array(perm, (void **)&A->perm, &A->device_bytes));
-    VEXB_TRY(upload_array(scol, (void **)&A->col, &A->device_bytes));
-    VEXB_TRY(upload_array(sval, &A->val, &A->device_bytes));
+    VEXB_TRY(upload_array(h.sptr, (void **)&S->slice_ptr, &S->device_bytes));
+    VEXB_TRY(upload_array(h.perm, (void **)&S->perm, &S->device_bytes));
+    VEXB_TRY(upload_array(scol, (void **)&S->col, &S->device_bytes));
+    VEXB_TRY(upload_array(sval, &S->val, &S->device_bytes));
     return VEXB_OK;
+}
+
+static int sell_upload(sell_strip *S, const sell_host &h, const void *val, int val_dtype, size_t comps) {
+    return val_dtype == VEXB_F64 ? sell_upload<double>(S, h, (const double *)val, comps)
+                                 : sell_upload<float>(S, h, (const float *)val, comps);
+}
+
+static void sell_free(sell_strip *S) {
+    cudaFree(S->slice_ptr); cudaFree(S->perm); cudaFree(S->col); cudaFree(S->val);
 }
 
 } // namespace vexb
@@ -142,39 +271,15 @@ extern "C" int vexb_bsr_create(int dev, void *stream, size_t nrows, size_t ncols
     VEXB_CHECK(out, "out is NULL");
     *out = nullptr;
     VEXB_CHECK(block >= 2 && block <= 4, "block size %d is not 2, 3 or 4", block);
-    VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
-    VEXB_CHECK(ptr_bytes == 4 || ptr_bytes == 8, "ptr_bytes must be 4 or 8");
-    VEXB_CHECK(col_bytes == 4 || col_bytes == 8, "col_bytes must be 4 or 8");
-    VEXB_CHECK(nrows == 0 || ptr, "ptr is NULL");
-    VEXB_CHECK(nrows < (size_t)INT32_MAX && ncols < (size_t)INT32_MAX, "block dimensions exceed 32-bit local indices");
-    const int64_t p0 = nrows ? read_index(ptr, ptr_bytes, 0) : 0;
-    const int64_t nnzb = nrows ? read_index(ptr, ptr_bytes, nrows) - p0 : 0;
-    VEXB_CHECK(nnzb >= 0 && nnzb < (int64_t)INT32_MAX - 64, "nnzb=%lld does not fit 32-bit row pointers", (long long)nnzb);
-    VEXB_CHECK(nnzb == 0 || (col && val), "col/val is NULL");
-    std::vector<int> rp(nrows + 1, 0), c((size_t)nnzb);
-    for (size_t i = 1; i <= nrows; ++i) {
-        const int64_t v = read_index(ptr, ptr_bytes, i) - p0;
-        VEXB_CHECK(v >= rp[i - 1] && v <= nnzb, "row pointers decrease at block row %zu", i);
-        rp[i] = (int)v;
-    }
-    for (size_t j = 0; j < (size_t)nnzb; ++j) {
-        const int64_t cj = read_index(col, col_bytes, j);
-        VEXB_CHECK(cj >= 0 && (size_t)cj < ncols, "block column %lld out of range at block %zu", (long long)cj, j);
-        c[j] = (int)cj;
-    }
-    std::vector<int> perm, sptr;
-    size_t slots = 0;
-    VEXB_CHECK(sell_layout(nrows, rp.data(), param("spmv.sell_sigma", 1024), perm, sptr, &slots),
-               "block strip too large for 32-bit slot offsets");
+    sell_host h;
+    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, val_dtype, "block ", h));
 
     DeviceGuard g(dev);
     if (!g.ok) VEXB_FAIL(VEXB_ERR_CUDA, "cannot select device %d", dev);
     vexb_bspmat *A = new vexb_bspmat;
     A->dev = dev; A->block = block; A->val_dtype = val_dtype;
-    A->nrows = nrows; A->ncols = ncols; A->nnzb = (size_t)nnzb;
-    A->n_slices = sptr.size() - 1; A->n_slots = slots;
-    const int st = val_dtype == VEXB_F64 ? bsr_upload<double>(A, rp, c, (const double *)val, perm, sptr)
-                                         : bsr_upload<float>(A, rp, c, (const float *)val, perm, sptr);
+    A->nrows = nrows; A->ncols = ncols; A->nnzb = h.nnz;
+    const int st = sell_upload(A, h, val, val_dtype, (size_t)block * block);
     if (st != VEXB_OK) { vexb_bspmat_destroy(A); return st; }
     *out = A;
     return VEXB_OK;
@@ -184,7 +289,7 @@ extern "C" int vexb_bspmat_destroy(vexb_bspmat *A) {
     if (!A) return VEXB_OK;
     VEXB_RELEASE_GUARD();
     DeviceGuard g(A->dev);
-    cudaFree(A->slice_ptr); cudaFree(A->perm); cudaFree(A->col); cudaFree(A->val);
+    sell_free(A);
     delete A;
     return VEXB_OK;
 }
@@ -206,4 +311,54 @@ extern "C" int vexb_bspmv(int dev, void *stream, const vexb_bspmat *A, const voi
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     if (A->val_dtype == VEXB_F64) return bspmv_launch<double>(A, (cudaStream_t)stream, (const double *)x, (double *)y, alpha, append);
     return bspmv_launch<float>(A, (cudaStream_t)stream, (const float *)x, (float *)y, (float)alpha, append);
+}
+
+extern "C" int vexb_zsr_create(int dev, void *stream, size_t nrows, size_t ncols, const void *ptr, int ptr_bytes,
+                               const void *col, int col_bytes, const void *val, int val_dtype, vexb_zspmat **out) {
+    (void)stream;
+    // every argument is checked before a device is touched (tests/test_zsr_oracle.py runs these checks without one)
+    VEXB_CHECK(out, "out is NULL");
+    *out = nullptr;
+    sell_host h;
+    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, val_dtype, "", h));
+
+    DeviceGuard g(dev);
+    if (!g.ok) VEXB_FAIL(VEXB_ERR_CUDA, "cannot select device %d", dev);
+    vexb_zspmat *A = new vexb_zspmat;
+    A->dev = dev; A->val_dtype = val_dtype;
+    A->nrows = nrows; A->ncols = ncols; A->nnz = h.nnz;
+    const int st = sell_upload(A, h, val, val_dtype, 2);          // (re, im) of each entry: the bytes of std::complex<T>
+    if (st != VEXB_OK) { vexb_zspmat_destroy(A); return st; }
+    *out = A;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_zspmat_destroy(vexb_zspmat *A) {
+    if (!A) return VEXB_OK;
+    VEXB_RELEASE_GUARD();
+    DeviceGuard g(A->dev);
+    sell_free(A);
+    delete A;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_zspmat_get_info(const vexb_zspmat *A, vexb_zspmat_info *info) {
+    VEXB_CHECK(A && info, "NULL argument");
+    memset(info, 0, sizeof(*info));
+    info->nrows = A->nrows; info->ncols = A->ncols; info->nnz = A->nnz;
+    info->val_dtype = A->val_dtype;
+    info->n_slices = A->n_slices; info->n_slots = A->n_slots; info->device_bytes = A->device_bytes;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_zspmv(int dev, void *stream, const vexb_zspmat *A, const void *x, void *y, double alpha, int append) {
+    VEXB_CHECK(A, "matrix is NULL");
+    VEXB_CHECK(dev == A->dev, "matrix lives on device %d, not %d", A->dev, dev);
+    VEXB_CHECK(A->nrows == 0 || y, "y is NULL");
+    VEXB_CHECK(A->nnz == 0 || x, "x is NULL");
+    const size_t pair = A->val_dtype == VEXB_F64 ? 2 * sizeof(double) : 2 * sizeof(float);
+    VEXB_CHECK(A->nnz == 0 || (uintptr_t)x % pair == 0, "x is not aligned to one complex element (%zu bytes)", pair);
+    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
+    if (A->val_dtype == VEXB_F64) return zspmv_launch<double>(A, (cudaStream_t)stream, (const double *)x, (double *)y, alpha, append);
+    return zspmv_launch<float>(A, (cudaStream_t)stream, (const float *)x, (float *)y, (float)alpha, append);
 }

@@ -13,6 +13,9 @@ template <> __device__ __forceinline__ float t_mul<float>(float a, float b) { re
 template <class T> __device__ __forceinline__ T t_add(T a, T b);
 template <> __device__ __forceinline__ double t_add<double>(double a, double b) { return __dadd_rn(a, b); }
 template <> __device__ __forceinline__ float t_add<float>(float a, float b) { return __fadd_rn(a, b); }
+template <class T> __device__ __forceinline__ T t_sub(T a, T b);
+template <> __device__ __forceinline__ double t_sub<double>(double a, double b) { return __dsub_rn(a, b); }
+template <> __device__ __forceinline__ float t_sub<float>(float a, float b) { return __fsub_rn(a, b); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -48,6 +51,13 @@ __device__ __forceinline__ double ldg_keep(const double *p, uint64_t policy) {
 }
 __device__ __forceinline__ float ldg_keep(const float *p, uint64_t policy) {
     float v; asm volatile("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(policy)); return v;
+}
+// (re, im) of a complex element in one 16- or 8-byte load; p must be aligned to the pair
+__device__ __forceinline__ double2 ldg_keep(const double2 *p, uint64_t policy) {
+    double2 v; asm volatile("ld.global.nc.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(v.x), "=d"(v.y) : "l"(p), "l"(policy)); return v;
+}
+__device__ __forceinline__ float2 ldg_keep(const float2 *p, uint64_t policy) {
+    float2 v; asm volatile("ld.global.nc.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(v.x), "=f"(v.y) : "l"(p), "l"(policy)); return v;
 }
 __device__ __forceinline__ int ldg_stream(const int *p, uint64_t policy) {
     int v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(policy)); return v;
