@@ -258,7 +258,7 @@ template <class T>
 __global__ void __launch_bounds__(kDirectThreads, 5) csr_direct_kernel(const int2 *__restrict__ tile, const int *__restrict__ rowptr,
                                                                         const int *__restrict__ col, const T *__restrict__ val,
                                                                         const T *__restrict__ x, T *y, T alpha, int append,
-                                                                        const int *__restrict__ row_ids) {
+                                                                        int tile_nnz, const int *__restrict__ row_ids) {
     extern __shared__ __align__(16) unsigned char smem[];
     T *prod = reinterpret_cast<T *>(smem);
     const int tid = threadIdx.x;
@@ -268,8 +268,9 @@ __global__ void __launch_bounds__(kDirectThreads, 5) csr_direct_kernel(const int
     if (nr <= 0) return;
     const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
 
-    if (cnt > kDirectThreads * kDirectPerThread) {
-        // one long row: the whole CTA strides over it
+    if (cnt > tile_nnz) {
+        // one long row (build() gives a row longer than tile_nnz a tile of its own; prod holds only tile_nnz
+        // products): the whole CTA strides over it
         T s = T(0);
         for (int j = j0 + tid; j < j0 + cnt; j += kDirectThreads) s = t_add<T>(s, t_mul<T>(ldg_stream(val + j, stream), ldg_keep(x + ldg_stream(col + j, stream), keep)));
 #pragma unroll
@@ -1407,7 +1408,7 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
     } else if (A->fmt == VEXB_FMT_CSR && variant == 2 && A->tile_nnz <= (size_t)kDirectThreads * kDirectPerThread) {
         const size_t smem = std::max<size_t>(A->tile_nnz, 64) * sizeof(T);
         csr_direct_kernel<T><<<(unsigned)A->n_tiles, kDirectThreads, smem, st>>>(A->tile, A->rowptr, A->col, (const T *)A->val, x, y,
-                                                                                alpha, append, A->row_ids);
+                                                                                alpha, append, (int)A->tile_nnz, A->row_ids);
         VEXB_LAUNCHED();
     } else if (A->fmt == VEXB_FMT_CSR && variant == 1) {
         long stages = param("spmv.stages", 4);
