@@ -402,6 +402,15 @@ typedef enum {
                              shared memory, products added in storage order (same bits as the reference loop).  What
                              VEXB_FMT_AUTO picks for rows too irregular for hybrid ELL. */
 } vexb_spfmt;
+/* Flag ORed into `fmt` of vexb_csr_create / vexb_dspmat_create, double values only: store each value as (float)v (round
+ * to nearest even; a finite value that would round to +-inf is rejected with VEXB_ERR_INVALID).  x, y, every product
+ * double(v_f) * x_j and every sum stay double, in the order of the double strip: y has the bits of the double strip built
+ * from the rounded values, with the same layout (format, width, encoding, classes, tiles).  Only the per-entry value
+ * arrays shrink (sliced ELL, hybrid ELL and its CSR tail, CSR); row-class and row-pattern strips keep their small tables
+ * in double.  CSR strips run "spmv.kernel" 3 and 4 only (VEXB_ERR_UNSUPPORTED for the others).  Readers without a
+ * float-valued kernel refuse such strips: vexb_spmv_multi multiplies one vector at a time, vexb_dspmat_inline_strip gives
+ * NULL, vexb_dspmat_halo_connect* and vexb_dspmat_apply_dot return VEXB_ERR_UNSUPPORTED. */
+#define VEXB_FMT_VALUES_F32 0x100
 /* Host-only: the row patterns VEXB_FMT_PATTERNS would use.  *n_patterns = number of distinct rows; idx (optional,
  * nrows entries) = pattern of each row.  Returns VEXB_ERR_UNSUPPORTED when there are more than max_patterns. */
 int vexb_csr_row_patterns(size_t nrows, const void *ptr, int ptr_bytes, const void *col, int col_bytes,
@@ -429,9 +438,13 @@ typedef struct {
     int32_t ell_classes;                          /* HELL: number of row classes ("spmv.ell_classes": one class byte per row,
                                                      slot masks and values in a table of at most 256 classes); 0 = values
                                                      stored per slot */
+    int32_t val_bytes;                            /* bytes per stored value of the per-entry value arrays: 8 (double),
+                                                     4 (float, or double values with VEXB_FMT_VALUES_F32); 0 for row-class
+                                                     and row-pattern strips, whose tables hold the values */
 } vexb_spmat_info;
 int vexb_spmat_get_info(const vexb_spmat *A, vexb_spmat_info *info);
-/* Copy the HELL arrays back (parity with hybrid_ell.inl:132-193); any pointer may be NULL. */
+/* Copy the HELL arrays back (parity with hybrid_ell.inl:132-193); any pointer may be NULL.  Values come back in the
+ * strip's value type: double for VEXB_FMT_VALUES_F32 strips (the rounded values). */
 int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, void *ell_val,
                              int64_t *csr_ptr, int32_t *csr_col, void *csr_val);
 /* y (=|+=) alpha * A x     (csr.inl:188-209: append ? "+=" : "=") */
@@ -564,7 +577,8 @@ typedef struct {
     vexb_spmat_info loc, rem;
 } vexb_dspmat_info;
 int vexb_dspmat_get_info(const vexb_dspmat *A, vexb_dspmat_info *info);
-/* Split tables back on the host for parity with csr.inl:70-112 (any pointer may be NULL). */
+/* Split tables back on the host for parity with csr.inl:70-112 (any pointer may be NULL); VEXB_FMT_VALUES_F32 parts give
+ * the rounded values, as double. */
 int vexb_dspmat_download_split(const vexb_dspmat *A, int64_t *loc_ptr, int64_t *loc_col, void *loc_val,
                                int64_t *rem_ptr, int64_t *rem_col, void *rem_val);
 /* The part's strip for use as a VEXB_TERM_SPMV terminal: set when the part has no ghost columns and its rows are

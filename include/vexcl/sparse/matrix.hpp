@@ -56,10 +56,11 @@ class single_device_matrix {
             VEXB_CHECKED(vexb_spmv(q[0].ordinal(), q[0].raw(), A.get(), x(0).raw(), y(0).raw(), static_cast<double>(alpha), append));
         }
 
-        /// The strip when a generated kernel can walk its rows (CSR / hybrid ELL), else NULL.
+        /// The strip when a generated kernel can walk its rows (CSR / hybrid ELL with values of the vector type), else NULL.
         const vexb_spmat* inline_strip(unsigned = 0) const {
             vexb_spmat_info i;
             if (!A || vexb_spmat_get_info(A.get(), &i) != VEXB_OK) return nullptr;
+            if (i.val_dtype == VEXB_F64 && i.val_bytes == 4) return nullptr;      // VEXB_FMT_VALUES_F32
             return (i.fmt == VEXB_FMT_CSR || i.fmt == VEXB_FMT_HELL) ? A.get() : nullptr;
         }
 

@@ -18,6 +18,7 @@ SET, ADD, SUB, MUL, DIV, MOD, AND, OR, XOR, LSH, RSH = range(11)
 SUM, SUM_KAHAN, MAX, MIN, MINMAX = range(5)
 TERM_VEC, TERM_SCALAR, TERM_INDEX, TERM_DSCALAR, TERM_SPMV = range(5)
 FMT_AUTO, FMT_CSR, FMT_HELL, FMT_PATTERNS, FMT_SELL = range(5)
+FMT_VALUES_F32 = 0x100          # ORed into fmt: double values stored as float, double vectors and sums
 MAX_TERMS, MAX_CODE, MAX_STACK = 16, 64, 12
 
 _OPS = ("TERM CVT NEG LNOT ADD SUB MUL DIV MOD BAND BOR BXOR SHL SHR LT GT LE GE EQ NE LAND LOR SELECT "
@@ -54,7 +55,7 @@ class SpmatInfo(C.Structure):
                 ("val_dtype", C.c_int32), ("ell_width", C.c_size_t), ("ell_pitch", C.c_size_t),
                 ("csr_tail_nnz", C.c_size_t), ("n_tiles", C.c_size_t), ("tile_nnz", C.c_size_t),
                 ("device_bytes", C.c_size_t), ("ell_col_bytes", C.c_int32),
-                ("ell_classes", C.c_int32)]
+                ("ell_classes", C.c_int32), ("val_bytes", C.c_int32)]
 
 
 class BspmatInfo(C.Structure):

@@ -381,6 +381,7 @@ static bool is_neighbour(const vexb_dspmat *A, int p) { return p != A->part && (
 
 extern "C" int vexb_dspmat_halo_connect(vexb_dspmat *A, const void *handles) {
     VEXB_CHECK(A && handles, "NULL argument");
+    if (A->values_f32) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no peer-memory halo for float values (VEXB_FMT_VALUES_F32): NCCL or copies");
     VEXB_TRY(halo_prepare(A));
     HaloLink *h = A->halo;
     DeviceGuard g(A->dev); VEXB_CHECK(g.ok, "cannot select device %d", A->dev);
@@ -398,6 +399,8 @@ extern "C" int vexb_dspmat_halo_connect(vexb_dspmat *A, const void *handles) {
 extern "C" int vexb_dspmat_halo_connect_local(int nlocal, vexb_dspmat *const *parts) {
     VEXB_CHECK(nlocal >= 1 && parts, "bad arguments");
     VEXB_CHECK(nlocal == parts[0]->nparts, "every part must be local (%d of %d given)", nlocal, parts[0]->nparts);
+    for (int a = 0; a < nlocal; ++a)
+        if (parts[a] && parts[a]->values_f32) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no peer-memory halo for float values (VEXB_FMT_VALUES_F32): NCCL or copies");
     for (int a = 0; a < nlocal; ++a) {
         VEXB_CHECK(parts[a] && parts[a]->part == a, "parts must be passed in order");
         for (int b = a + 1; b < nlocal; ++b) VEXB_CHECK(parts[a]->dev != parts[b]->dev, "the peer-memory halo needs distinct devices");

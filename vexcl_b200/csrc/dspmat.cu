@@ -59,7 +59,6 @@ extern "C" int vexb_dspmat_create(int dev, void *stream, int part, const vexb_ha
     VEXB_CHECK(col_bytes == 4 || col_bytes == 8, "col_bytes must be 4 or 8");
     VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
     VEXB_CHECK(nrows == 0 || ptr, "ptr is NULL");
-    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
 
     const size_t col_begin = plan->col_part[part], col_end = plan->col_part[part + 1];
     const std::vector<int64_t> &ghost = plan->ghost[part];
@@ -68,9 +67,15 @@ extern "C" int vexb_dspmat_create(int dev, void *stream, int part, const vexb_ha
     const int64_t nnz = nrows ? read_index(ptr, ptr_bytes, nrows) - p0 : 0;
     VEXB_CHECK(nnz == 0 || (col && val), "col/val is NULL");
     VEXB_CHECK(nnz < (int64_t)INT32_MAX - 64, "strip nnz does not fit 32-bit row pointers");
+    // format, flag, and values under the flag, before a device is touched; every strip below gets the rounded values
+    std::vector<double> rounded;
+    VEXB_TRY(check_fmt_flags(fmt, val_dtype, val, nnz > 0 ? (size_t)nnz : 0, rounded));
+    if (fmt & VEXB_FMT_VALUES_F32) val = rounded.data();
+    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
 
     auto *A = new vexb_dspmat();
     A->dev = dev; A->part = part; A->nparts = plan->nparts; A->val_dtype = val_dtype;
+    A->values_f32 = (fmt & VEXB_FMT_VALUES_F32) != 0;
     A->nrows = nrows; A->ncols_local = col_end - col_begin; A->n_ghost = ghost.size();
     A->send_counts = plan->send_counts[part]; A->recv_counts = plan->recv_counts[part];
     A->ghost_counts.resize(plan->nparts); A->land_off.assign(plan->nparts, 0);
@@ -167,8 +172,9 @@ extern "C" int vexb_dspmat_create(int dev, void *stream, int part, const vexb_ha
             }
             st = halo_set_boundary(A, bids, wb, mcol, mval.data());
         }
-        if (st == VEXB_OK) st = spmat_from_csr(dev, nrows, A->ncols_local, brow, bcol, bval.data(), val_dtype, VEXB_FMT_CSR, &bids, &A->bnd);
-        if (st == VEXB_OK) st = spmat_from_csr(dev, nrows, A->n_ghost, rrow, rcol, rval.data(), val_dtype, VEXB_FMT_CSR, &rids, &A->rem);
+        const int bfmt = VEXB_FMT_CSR | (fmt & VEXB_FMT_VALUES_F32);
+        if (st == VEXB_OK) st = spmat_from_csr(dev, nrows, A->ncols_local, brow, bcol, bval.data(), val_dtype, bfmt, &bids, &A->bnd);
+        if (st == VEXB_OK) st = spmat_from_csr(dev, nrows, A->n_ghost, rrow, rcol, rval.data(), val_dtype, bfmt, &rids, &A->rem);
     }
     if (st == VEXB_OK && plan->nparts <= VEXB_MAX_HALO_PARTS) st = halo_prepare(A);
     if (st != VEXB_OK) { vexb_dspmat_destroy(A); return st; }
@@ -225,8 +231,9 @@ extern "C" int vexb_dspmat_download_split(const vexb_dspmat *A, int64_t *loc_ptr
 extern "C" int vexb_dspmat_inline_strip(const vexb_dspmat *A, const vexb_spmat **strip) {
     VEXB_CHECK(A && strip, "NULL argument");
     const vexb_spmat *S = A->loc;
+    // the generated row loop reads values of the vector type: float-valued strips are multiplied into a temporary instead
     const bool ok = S && !A->n_ghost && !A->bnd && !A->rem && !S->row_ids && S->y_offset == 0 && S->nrows_stored == A->nrows &&
-                    (S->fmt == VEXB_FMT_CSR || S->fmt == VEXB_FMT_HELL) && S->d_desc && !param("spmv.no_inline", 0);
+                    (S->fmt == VEXB_FMT_CSR || S->fmt == VEXB_FMT_HELL) && !S->val_f32 && S->d_desc && !param("spmv.no_inline", 0);
     *strip = ok ? S : nullptr;
     return VEXB_OK;
 }
@@ -381,6 +388,7 @@ extern "C" int vexb_dspmat_apply_dot(int nlocal, vexb_dspmat *const *parts, void
         const vexb_spmat *S = parts[k]->loc;
         if (!c || !S || S->fmt != VEXB_FMT_HELL || S->nnz == 0 || param("dspmat.no_peer_halo", 0) || param("dspmat.no_fused_dot", 0))
             VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "fused product + dot needs the peer-memory halo and a hybrid-ELL interior strip on every part");
+        if (parts[k]->values_f32) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no fused product + dot for float values (VEXB_FMT_VALUES_F32)");
         VEXB_CHECK(parts[k]->nparts == 1 || (peers && peers[k]), "part %d: a peer group is needed to combine the dot across GPUs", k);
     }
     for (int k = 0; k < nlocal; ++k)

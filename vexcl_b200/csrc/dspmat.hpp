@@ -8,6 +8,7 @@ struct vexb_peer;
 
 struct vexb_dspmat {
     int dev = 0, part = 0, nparts = 1, val_dtype = VEXB_F64;
+    bool values_f32 = false;        // created with VEXB_FMT_VALUES_F32: no peer-memory halo, no fused product + dot
     size_t nrows = 0, ncols_local = 0, n_ghost = 0, n_send = 0;
     vexb_spmat *loc = nullptr;      // rows without ghost entries (all rows when there are no ghosts)
     vexb_spmat *bnd = nullptr;      // local entries of the rows that also have ghost entries (row-compressed)

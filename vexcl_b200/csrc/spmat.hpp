@@ -32,6 +32,7 @@ struct vexb_spmat {
     int dev = 0;
     int fmt = VEXB_FMT_CSR;
     int val_dtype = VEXB_F64;
+    bool val_f32 = false;          // VEXB_FMT_VALUES_F32: val, sell_val, ell_val and tail_val hold float (x, y, sums: double)
     size_t nrows = 0, ncols = 0, nnz = 0;
     // CSR stream
     void *val = nullptr; int *col = nullptr; int *rowptr = nullptr; int2 *tile = nullptr;
@@ -81,6 +82,11 @@ struct SpmvDesc {
 namespace vexb {
 // Build a strip from 32-bit host CSR.  row_ids (optional) maps stored row r to its y index;
 // nrows is then the length of y and rowptr.size()-1 the number of stored rows.
+// fmt may carry VEXB_FMT_VALUES_F32; val must then already be rounded to float (round_values_f32).
 int spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &rowptr, std::vector<int> &col,
                    const void *val, int val_dtype, int fmt, const std::vector<int> *row_ids, vexb_spmat **out);
+// Checks the flag bits of `fmt` against val_dtype and, with VEXB_FMT_VALUES_F32, fills `rounded` with double(float(v)) of
+// the n values (exact both ways, as numpy's astype(float32)); VEXB_ERR_INVALID when a finite value rounds to +-inf.
+// Host only: the create functions call it before they touch a device.
+int check_fmt_flags(int fmt, int val_dtype, const void *val, size_t n, std::vector<double> &rounded);
 }

@@ -481,13 +481,15 @@ constexpr int kEllClassRows = 2;
 // In bench.py (400 W card) 132 blocks cost configs[3] less than 528 (+1.4 % against +3.9 %) for the same gain on configs[2].
 constexpr int kEllClassPrefetchBlocks = 132;
 
-template <class T, int W, class C>
+// V: stored value type (hell_row_sum); float under double vectors for VEXB_FMT_VALUES_F32 strips, which never use row classes.
+template <class T, int W, class C, class V = T>
 __global__ void __launch_bounds__(256) hell_kernel(size_t n, size_t pitch, int w_dyn, const C *__restrict__ ell_col, const EllShifts shift,
-                                                    const T *__restrict__ ell_val, const int *__restrict__ tail_ptr,
-                                                    const int *__restrict__ tail_col, const T *__restrict__ tail_val,
+                                                    const V *__restrict__ ell_val, const int *__restrict__ tail_ptr,
+                                                    const int *__restrict__ tail_col, const V *__restrict__ tail_val,
                                                     const T *__restrict__ x, T *y, T alpha, int append,
                                                     const int *__restrict__ row_ids, int prefetch_blocks) {
     if constexpr (std::is_same<C, EllClass>::value) {
+        static_assert(std::is_same<T, V>::value, "row classes keep their table in the vector type");
         // Row classes: a row moves 17 bytes (class, x, y), too few for one row per thread to keep enough bytes in flight.
         // A thread takes kEllClassRows rows, a block apart, so at every sub-step a warp's lanes hold consecutive rows
         // (coalesced class bytes and y stores); rows past the end repeat row n-1 and store nothing.
@@ -521,7 +523,7 @@ __global__ void __launch_bounds__(256) hell_kernel(size_t n, size_t pitch, int w
         const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
         if (i >= n) return;
         const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
-        const T sum = hell_row_sum<T, W, C>(i, pitch, w_dyn, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep);
+        const T sum = hell_row_sum<T, W, C, V>(i, pitch, w_dyn, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep);
         store_y<T>(y, row_ids ? (size_t)row_ids[i] : i, sum, alpha, append);
     }
 }
@@ -612,10 +614,10 @@ __global__ void __launch_bounds__(256) hell_multi_kernel(size_t n, size_t pitch,
 // neighbouring rows, i.e. addresses a row length apart: not coalesced per instruction, but every 32-byte sector a warp
 // touches is consumed completely by it over the row loop, so with L1 allocation (plain loads, no streaming hint) DRAM
 // traffic stays at the algorithmic figure.  No shared memory, no barrier, no tile descriptor: every thread always has
-// loads in flight, like hell_kernel.
-template <class T>
+// loads in flight, like hell_kernel.  V: stored value type, as in hell_kernel.
+template <class T, class V = T>
 __global__ void __launch_bounds__(256) csr_scalar_kernel(size_t n, const int *__restrict__ rowptr, const int *__restrict__ col,
-                                                          const T *__restrict__ val, const T *__restrict__ x, T *y, T alpha,
+                                                          const V *__restrict__ val, const T *__restrict__ x, T *y, T alpha,
                                                           int append, const int *__restrict__ row_ids) {
     const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
@@ -629,7 +631,7 @@ __global__ void __launch_bounds__(256) csr_scalar_kernel(size_t n, const int *__
         sum = t_add<T>(sum, t_mul<T>(v0, x0)); sum = t_add<T>(sum, t_mul<T>(v1, x1));
         sum = t_add<T>(sum, t_mul<T>(v2, x2)); sum = t_add<T>(sum, t_mul<T>(v3, x3));
     }
-    for (; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(val[j], __ldg(x + col[j])));
+    for (; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(T(val[j]), __ldg(x + col[j])));
     store_y<T>(y, row_ids ? (size_t)row_ids[r] : r, sum, alpha, append);
 }
 
@@ -678,9 +680,11 @@ __device__ __forceinline__ void warp_rows(const T *prod, const int *__restrict__
 // lanes per row for a tile of cnt nonzeros in nr rows
 __device__ __forceinline__ int warp_tile_group(int cnt, int nr) { return cnt <= 6 * nr ? 1 : cnt <= 24 * nr ? 4 : cnt <= 64 * nr ? 8 : 32; }
 
-template <class T>
-__global__ void __launch_bounds__(256, 4) csr_warp_kernel(const int2 *__restrict__ tile, int n_tiles, const int *__restrict__ rowptr,
-                                                           const int *__restrict__ col, const T *__restrict__ val,
+// V: stored value type, as in hell_kernel.  Float values under double vectors need more than the 64 registers of 4 CTAs
+// per SM (88 bytes of spills): that instantiation runs 3.
+template <class T, class V = T>
+__global__ void __launch_bounds__(256, std::is_same<T, V>::value ? 4 : 3) csr_warp_kernel(const int2 *__restrict__ tile, int n_tiles, const int *__restrict__ rowptr,
+                                                           const int *__restrict__ col, const V *__restrict__ val,
                                                            const T *__restrict__ x, T *y, T alpha, int append,
                                                            const int *__restrict__ row_ids) {
     __shared__ T prod_all[8][kWarpTileNnz];
@@ -697,7 +701,7 @@ __global__ void __launch_bounds__(256, 4) csr_warp_kernel(const int2 *__restrict
     int2 d0 = __ldg(tile + t), d1 = __ldg(tile + t + 1);                 // current
     int2 n0 = d0, n1 = d1;                                               // next
     { const int tn = t + total_warps; if (tn < n_tiles) { n0 = __ldg(tile + tn); n1 = __ldg(tile + tn + 1); } }
-    int c[kWarpPer]; T v[kWarpPer]; int pa[2], pb[2];
+    int c[kWarpPer]; V v[kWarpPer]; int pa[2], pb[2];
     auto issue = [&](const int2 &e0, const int2 &e1) {
         const int r0 = e0.x, nr = e1.x - e0.x, j0 = e0.y, cnt = e1.y - e0.y;
         if (cnt > kWarpTileNnz || nr <= 0) return;
@@ -722,21 +726,37 @@ __global__ void __launch_bounds__(256, 4) csr_warp_kernel(const int2 *__restrict
         if (cnt > kWarpTileNnz) {
             // one long row: the warp strides over it
             T s = T(0);
-            for (int j = j0 + lane; j < j0 + cnt; j += 32) s = t_add<T>(s, t_mul<T>(ldg_stream(val + j, stream), ldg_keep(x + ldg_stream(col + j, stream), keep)));
+            for (int j = j0 + lane; j < j0 + cnt; j += 32) s = t_add<T>(s, t_mul<T>(T(ldg_stream(val + j, stream)), ldg_keep(x + ldg_stream(col + j, stream), keep)));
 #pragma unroll
             for (int off = 16; off > 0; off >>= 1) s = t_add<T>(s, __shfl_down_sync(0xffffffffu, s, off));
             if (lane == 0) store_y<T>(y, row_ids ? (size_t)row_ids[r0] : (size_t)r0, s, alpha, append);
             if (tn < n_tiles) issue(n0, n1);
         } else if (nr > 0) {
+            if constexpr (std::is_same<T, V>::value) {
 #pragma unroll
-            for (int k = 0; k < kWarpPer; ++k) {
-                const int j = lane + 32 * k;
-                if (j < cnt) v[k] = t_mul<T>(v[k], ldg_keep(x + c[k], keep));
-            }
+                for (int k = 0; k < kWarpPer; ++k) {
+                    const int j = lane + 32 * k;
+                    if (j < cnt) v[k] = t_mul<T>(v[k], ldg_keep(x + c[k], keep));
+                }
 #pragma unroll
-            for (int k = 0; k < kWarpPer; ++k) {
-                const int j = lane + 32 * k;
-                if (j < cnt) prod[j] = v[k];
+                for (int k = 0; k < kWarpPer; ++k) {
+                    const int j = lane + 32 * k;
+                    if (j < cnt) prod[j] = v[k];
+                }
+            } else {
+                // float values under double vectors: the products cannot go back over the values, they go straight to
+                // shared memory once all gathers are out (a third register array would spill)
+                T xv[kWarpPer];
+#pragma unroll
+                for (int k = 0; k < kWarpPer; ++k) {
+                    const int j = lane + 32 * k;
+                    if (j < cnt) xv[k] = ldg_keep(x + c[k], keep);
+                }
+#pragma unroll
+                for (int k = 0; k < kWarpPer; ++k) {
+                    const int j = lane + 32 * k;
+                    if (j < cnt) prod[j] = t_mul<T>(T(v[k]), xv[k]);
+                }
             }
             const int qa[2] = {pa[0], pa[1]}, qb[2] = {pb[0], pb[1]};
             __syncwarp();
@@ -909,10 +929,10 @@ __global__ void __launch_bounds__(256, 3) csr_ring_kernel(const int2 *__restrict
 // as wide as THEIR longest row, and rows are sorted by length inside windows of sigma rows first, so a slice's rows are
 // nearly equally long.  Products are added in storage order: same bits as the reference loop (csr.inl:163-170).
 // C = short: a stored column is its distance from (the lane's row + shift), -32768 = padding (banded strips: 10 instead
-// of 12 bytes per slot); C = int: the column itself, -1 = padding.
-template <class T, class C>
+// of 12 bytes per slot); C = int: the column itself, -1 = padding.  V: stored value type, as in hell_kernel.
+template <class T, class C, class V = T>
 __global__ void __launch_bounds__(256) sell_kernel(size_t n_slices, const int *__restrict__ slice_ptr, const int *__restrict__ perm,
-                                                   const C *__restrict__ col, int shift, const T *__restrict__ val,
+                                                   const C *__restrict__ col, int shift, const V *__restrict__ val,
                                                    const T *__restrict__ x, T *y, T alpha, int append,
                                                    const int *__restrict__ row_ids, size_t y_offset) {
     const size_t s = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -922,18 +942,18 @@ __global__ void __launch_bounds__(256) sell_kernel(size_t n_slices, const int *_
     const int base = __ldg(slice_ptr + s), w = (__ldg(slice_ptr + s + 1) - base) >> 5;
     const int r = ldg_stream(perm + s * 32 + lane, stream);
     const C *cp = col + base + lane;
-    const T *vp = val + base + lane;
+    const V *vp = val + base + lane;
     const size_t rr = r >= 0 ? (size_t)r : 0;
     T sum = T(0);
     int k = 0;
     for (; k + 4 <= w; k += 4) {                          // 4 slots: 8 coalesced loads, then 4 gathers, in flight together
-        int c[4]; T v[4], xv[4];
+        int c[4]; V v[4]; T xv[4];
 #pragma unroll
         for (int u = 0; u < 4; ++u) { c[u] = ell_column(ldg_stream(cp + (k + u) * 32, stream), rr, shift); v[u] = ldg_stream(vp + (k + u) * 32, stream); }
 #pragma unroll
         for (int u = 0; u < 4; ++u) xv[u] = c[u] != -1 ? ldg_keep(x + c[u], keep) : T(0);
 #pragma unroll
-        for (int u = 0; u < 4; ++u) if (c[u] != -1) sum = t_add<T>(sum, t_mul<T>(v[u], xv[u]));
+        for (int u = 0; u < 4; ++u) if (c[u] != -1) sum = t_add<T>(sum, t_mul<T>(T(v[u]), xv[u]));
     }
     for (; k < w; ++k) {
         const int c = ell_column(ldg_stream(cp + k * 32, stream), rr, shift);
@@ -959,6 +979,15 @@ static int upload(std::vector<T> &h, size_t pad, void **d, size_t *bytes_acc) {
     if (!h.empty()) VEXB_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
     *bytes_acc += n * sizeof(T);
     return VEXB_OK;
+}
+
+// A per-entry value array of the strip: as built, or as float on VEXB_FMT_VALUES_F32 strips (exact: the values were
+// rounded to float by check_fmt_flags).
+template <class T>
+static int upload_values(vexb_spmat *A, std::vector<T> &h, size_t pad, void **d) {
+    if (!A->val_f32) return upload(h, pad, d, &A->device_bytes);
+    std::vector<float> f(h.begin(), h.end());
+    return upload(f, pad, d, &A->device_bytes);
 }
 
 // Width of the ELL part: smallest w such that the rows wider than w are fewer
@@ -1062,6 +1091,7 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
                                A->val_dtype, &A->patterns) == VEXB_OK) {
                 A->fmt = VEXB_FMT_PATTERNS;
                 A->n_patterns = prow.size() - 1;
+                A->val_f32 = false;                                     // the unique-row table stays double
                 return VEXB_OK;
             }
             A->patterns = nullptr;
@@ -1132,7 +1162,7 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
             }
         }
         if (!narrow) VEXB_TRY(upload(scol, 32, (void **)&A->sell_col, &A->device_bytes));
-        VEXB_TRY(upload(sval, 32, &A->sell_val, &A->device_bytes));
+        VEXB_TRY(upload_values(A, sval, 32, &A->sell_val));
         return VEXB_OK;
     }
     if (fmt == VEXB_FMT_CSR) {
@@ -1195,10 +1225,11 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
         A->csr_variant = (mean <= 8.0 && (double)maxw <= 2.0 * mean + 2.0) ? 3 : 4;
         // CTA tiles with the x window in shared memory stay opt-in (spmv.kernel = 6 or spmv.auto_window = 1): the
         // one-shot CTA (copy, wait, multiply, add up) costs more than the L1 tag lookups it saves
-        if (A->csr_variant == 4 && param("spmv.auto_window", 0) && A->n_windowed_tiles * 10 >= A->n_tiles * 9) A->csr_variant = 6;
+        // (float-valued strips: 3 and 4 only)
+        if (A->csr_variant == 4 && !A->val_f32 && param("spmv.auto_window", 0) && A->n_windowed_tiles * 10 >= A->n_tiles * 9) A->csr_variant = 6;
         VEXB_TRY(upload(rowptr, 16, (void **)&A->rowptr, &A->device_bytes));
         VEXB_TRY(upload(col, 16, (void **)&A->col, &A->device_bytes));
-        VEXB_TRY(upload(val, 16, &A->val, &A->device_bytes));
+        VEXB_TRY(upload_values(A, val, 16, &A->val));
     } else {
         const size_t w = hell_width(rowptr, n);
         const size_t pitch = (n + 15) / 16 * 16;            // alignup(n, 16): hybrid_ell.inl:60
@@ -1297,6 +1328,7 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
                     (A->ell_nclass = ell_row_classes(pitch, w, mask, eval, cid, ctab)) > 0) {
                     // padding slots gather x at a column clamped to the strip's largest one (ell_class_column)
                     A->ell_shifts.x_max = *std::max_element(ecol.begin(), ecol.end());
+                    A->val_f32 = false;                         // the class table and the CSR tail stay double
                     VEXB_TRY(upload(cid, 0, (void **)&A->ell_class, &A->device_bytes));
                     VEXB_TRY(upload(ctab, 0, &A->ell_ctab, &A->device_bytes));
                 } else {
@@ -1318,17 +1350,20 @@ static int build(vexb_spmat *A, std::vector<int> &rowptr, std::vector<int> &col,
             }
         }
         if (!A->ell_col16 && !A->ell_mask && !A->ell_class) VEXB_TRY(upload(ecol, 0, (void **)&A->ell_col, &A->device_bytes));
-        if (!A->ell_class) VEXB_TRY(upload(eval, 0, &A->ell_val, &A->device_bytes));
+        if (!A->ell_class) VEXB_TRY(upload_values(A, eval, 0, &A->ell_val));
         if (A->tail_nnz) {
             VEXB_TRY(upload(tptr, 0, (void **)&A->tail_ptr, &A->device_bytes));
             VEXB_TRY(upload(tcol, 0, (void **)&A->tail_col, &A->device_bytes));
-            VEXB_TRY(upload(tval, 0, &A->tail_val, &A->device_bytes));
+            VEXB_TRY(upload_values(A, tval, 0, &A->tail_val));
         }
     }
     return VEXB_OK;
 }
 
-template <class T>
+// V: stored value type of the per-entry value arrays (float on VEXB_FMT_VALUES_F32 strips under double vectors).  Such
+// strips are sliced ELL, hybrid ELL without row classes, or CSR run by variant 3 or 4: the other kernels are only ever
+// launched with V = T.
+template <class T, class V = T>
 static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T alpha, int append) {
     // A strip touches exactly its stored rows: all of y[0, nrows) normally, y[row_ids[r]] for a
     // row-compressed strip, y[y_offset + r] for a strip that covers a contiguous sub-range.
@@ -1344,10 +1379,10 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
     if (A->fmt == VEXB_FMT_SELL) {
         // y was advanced by y_offset above; the kernel adds nothing more
         const unsigned sb = (unsigned)((A->n_slices + 7) / 8);
-        if (A->sell_col16) sell_kernel<T, short><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col16, A->sell_shift, (const T *)A->sell_val,
-                                                                   x, y, alpha, append, A->row_ids, 0);
-        else sell_kernel<T, int><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col, 0, (const T *)A->sell_val,
-                                                   x, y, alpha, append, A->row_ids, 0);
+        if (A->sell_col16) sell_kernel<T, short, V><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col16, A->sell_shift, (const V *)A->sell_val,
+                                                                      x, y, alpha, append, A->row_ids, 0);
+        else sell_kernel<T, int, V><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col, 0, (const V *)A->sell_val,
+                                                      x, y, alpha, append, A->row_ids, 0);
         VEXB_LAUNCHED();
         return VEXB_OK;
     }
@@ -1355,6 +1390,8 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
     //              4 = warp tiles, 5 = warp rings (TMA), 6 = CTA tiles with the x window in shared memory; unset (-1) = the strip's own choice (build(): 3 for short even rows, else 4)
     long variant = param("spmv.kernel", param("spmv.pipeline", 0) ? 1 : -1);
     if (variant < 0) variant = A->csr_variant;
+    if (!std::is_same<T, V>::value && A->fmt == VEXB_FMT_CSR && variant != 3 && variant != 4)
+        VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "spmv.kernel = %ld has no float-valued instantiation: CSR strips with float values run 3 and 4", variant);
     if (A->fmt == VEXB_FMT_CSR && variant == 6 && (reinterpret_cast<uintptr_t>(x) & 15) != 0) variant = 4;   // the window copy needs a 16-byte aligned x
     if (A->fmt == VEXB_FMT_CSR && variant == 6) {
         const size_t smem = (A->tile_nnz + 8) * sizeof(T) + (A->xwin + 4) * sizeof(T) + (A->tile_nnz + 8) * 4 + (A->tile_rows + 12) * 4 + 16;
@@ -1394,16 +1431,16 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
         const int ti = sizeof(T) == 8 ? 0 : 1;
         if (!per_sm[ti].load()) {
             int v = 0;
-            VEXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, csr_warp_kernel<T>, 256, 0));
+            VEXB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, csr_warp_kernel<T, V>, 256, 0));
             per_sm[ti].store(v > 0 ? v : 1);
         }
         const long cap = param("spmv.ctas_per_sm", 0);
         const size_t resident = (size_t)(cap > 0 && cap < per_sm[ti].load() ? cap : per_sm[ti].load()) * (size_t)sm_count(A->dev);
         const size_t grid = std::min((A->n_wtiles + 7) / 8, resident);
-        csr_warp_kernel<T><<<(unsigned)grid, 256, 0, st>>>(A->wtile, (int)A->n_wtiles, A->rowptr, A->col, (const T *)A->val, x, y, alpha, append, A->row_ids);
+        csr_warp_kernel<T, V><<<(unsigned)grid, 256, 0, st>>>(A->wtile, (int)A->n_wtiles, A->rowptr, A->col, (const V *)A->val, x, y, alpha, append, A->row_ids);
         VEXB_LAUNCHED();
     } else if (A->fmt == VEXB_FMT_CSR && variant == 3) {
-        csr_scalar_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, A->rowptr, A->col, (const T *)A->val, x, y, alpha, append, A->row_ids);
+        csr_scalar_kernel<T, V><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, A->rowptr, A->col, (const V *)A->val, x, y, alpha, append, A->row_ids);
         VEXB_LAUNCHED();
     } else if (A->fmt == VEXB_FMT_CSR && variant == 2 && A->tile_nnz <= (size_t)kDirectThreads * kDirectPerThread) {
         const size_t smem = std::max<size_t>(A->tile_nnz, 64) * sizeof(T);
@@ -1448,17 +1485,17 @@ static int spmv_launch(const vexb_spmat *A, cudaStream_t st, const T *x, T *y, T
     } else {
         const unsigned blocks = (unsigned)((n + 255) / 256);
 #define HL(W) do { \
-            if (A->ell_col16) hell_kernel<T, W, short><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col16, A->ell_shifts, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0); \
-            else hell_kernel<T, W, int><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col, EllShifts{}, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0); } while (0)
-#define HD(W) hell_kernel<T, W, EllDiag><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_mask, A->ell_shifts, \
-                  (const T *)A->ell_val, A->tail_ptr, A->tail_col, (const T *)A->tail_val, x, y, alpha, append, A->row_ids, 0)
+            if (A->ell_col16) hell_kernel<T, W, short, V><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col16, A->ell_shifts, \
+                  (const V *)A->ell_val, A->tail_ptr, A->tail_col, (const V *)A->tail_val, x, y, alpha, append, A->row_ids, 0); \
+            else hell_kernel<T, W, int, V><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col, EllShifts{}, \
+                  (const V *)A->ell_val, A->tail_ptr, A->tail_col, (const V *)A->tail_val, x, y, alpha, append, A->row_ids, 0); } while (0)
+#define HD(W) hell_kernel<T, W, EllDiag, V><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_mask, A->ell_shifts, \
+                  (const V *)A->ell_val, A->tail_ptr, A->tail_col, (const V *)A->tail_val, x, y, alpha, append, A->row_ids, 0)
 #define HC(W) hell_kernel<T, W, EllClass><<<(unsigned)((n + 256 * kEllClassRows - 1) / (256 * kEllClassRows)), 256, 0, st>>>( \
                   n, A->ell_pitch, (int)A->ell_width, A->ell_class, A->ell_shifts, (const T *)A->ell_ctab, A->tail_ptr, A->tail_col, \
                   (const T *)A->tail_val, x, y, alpha, append, A->row_ids, kEllClassPrefetchBlocks)
         if (A->ell_class) {
-            switch (A->ell_width) {   // = the widths build() gives row classes: those of slot masks
+            switch (A->ell_width) {   // = the widths build() gives row classes: those of slot masks (never float-valued)
                 case 3: HC(3); break; case 5: HC(5); break; case 7: HC(7); break;
                 default: VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no hell_kernel for row classes of width %zu", A->ell_width);
             }
@@ -1525,6 +1562,8 @@ int vexb::spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &
     auto *A = new vexb_spmat();
     A->dev = dev; A->val_dtype = val_dtype; A->nrows = nrows; A->ncols = ncols;
     A->nrows_stored = rowptr.size() - 1; A->nnz = (size_t)rowptr.back();
+    A->val_f32 = (fmt & VEXB_FMT_VALUES_F32) != 0;      // build() clears it where the values go to a table
+    fmt &= ~VEXB_FMT_VALUES_F32;
     const size_t nnz = A->nnz;
     int st = VEXB_OK;
     if (val_dtype == VEXB_F64) { std::vector<double> v((const double *)val, (const double *)val + nnz); st = build<double>(A, rowptr, col, v, fmt, row_ids == nullptr); }
@@ -1547,6 +1586,21 @@ int vexb::spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &
     }
     if (st != VEXB_OK) { vexb_spmat_destroy(A); return st; }
     *out = A;
+    return VEXB_OK;
+}
+
+int vexb::check_fmt_flags(int fmt, int val_dtype, const void *val, size_t n, std::vector<double> &rounded) {
+    const int base = fmt & ~VEXB_FMT_VALUES_F32;
+    VEXB_CHECK(base >= VEXB_FMT_AUTO && base <= VEXB_FMT_SELL, "bad format %d", fmt);
+    if (!(fmt & VEXB_FMT_VALUES_F32)) return VEXB_OK;
+    VEXB_CHECK(val_dtype == VEXB_F64, "VEXB_FMT_VALUES_F32 needs double values");
+    rounded.resize(n);
+    for (size_t j = 0; j < n; ++j) {
+        const double v = static_cast<const double *>(val)[j];
+        const float f = (float)v;                                     // round to nearest even
+        VEXB_CHECK(!std::isinf(f) || std::isinf(v), "value %g at entry %zu overflows float (VEXB_FMT_VALUES_F32)", v, j);
+        rounded[j] = (double)f;
+    }
     return VEXB_OK;
 }
 
@@ -1581,15 +1635,16 @@ extern "C" int vexb_csr_create(int dev, void *stream, size_t nrows, size_t ncols
     VEXB_CHECK(ptr_bytes == 4 || ptr_bytes == 8, "ptr_bytes must be 4 or 8");
     VEXB_CHECK(col_bytes == 4 || col_bytes == 8, "col_bytes must be 4 or 8");
     VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
-    VEXB_CHECK(fmt >= VEXB_FMT_AUTO && fmt <= VEXB_FMT_SELL, "bad format %d", fmt);
     VEXB_CHECK(nrows == 0 || ptr, "ptr is NULL");
     VEXB_CHECK(nrows < (size_t)INT32_MAX && ncols < (size_t)INT32_MAX, "strip dimensions exceed 32-bit local indices");
-    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
 
     const int64_t p0 = nrows ? read_index(ptr, ptr_bytes, 0) : 0;
     const int64_t nnz = nrows ? read_index(ptr, ptr_bytes, nrows) - p0 : 0;
     VEXB_CHECK(nnz >= 0 && nnz < (int64_t)INT32_MAX - 64, "strip nnz=%lld does not fit 32-bit row pointers", (long long)nnz);
     VEXB_CHECK(nnz == 0 || (col && val), "col/val is NULL");
+    std::vector<double> rounded;                                       // format, flag, and values under the flag
+    VEXB_TRY(check_fmt_flags(fmt, val_dtype, val, (size_t)nnz, rounded));
+    if (fmt & VEXB_FMT_VALUES_F32) val = rounded.data();
 
     std::vector<int> rp(nrows + 1), c((size_t)nnz);
     for (size_t i = 0; i <= nrows; ++i) {
@@ -1601,6 +1656,8 @@ extern "C" int vexb_csr_create(int dev, void *stream, size_t nrows, size_t ncols
         VEXB_CHECK(cj >= 0 && (size_t)cj < ncols, "column %lld out of range at nnz %zu", (long long)cj, j);
         c[j] = (int)cj;
     }
+    // every argument is checked before a device is touched
+    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     return spmat_from_csr(dev, nrows, ncols, rp, c, val, val_dtype, fmt, nullptr, out);
 }
 
@@ -1626,6 +1683,7 @@ extern "C" int vexb_spmat_get_info(const vexb_spmat *A, vexb_spmat_info *info) {
     info->device_bytes = A->device_bytes;
     info->ell_col_bytes = A->ell_mask || A->ell_class ? 0 : A->ell_col16 ? 2 : A->ell_col ? 4 : 0;
     info->ell_classes = (int32_t)A->ell_nclass;
+    info->val_bytes = A->patterns || A->ell_class ? 0 : A->val_f32 ? 4 : (int32_t)dtype_size(A->val_dtype);
     if (A->patterns) {
         vexb_ccsr_info ci;
         VEXB_TRY(vexb_ccsr_get_info(A->patterns, &ci));
@@ -1659,6 +1717,15 @@ extern "C" int vexb_csr_row_patterns(size_t nrows, const void *ptr, int ptr_byte
     *n_patterns = ok ? prow.size() - 1 : 0;
     if (ok && idx) std::memcpy(idx, id.data(), nrows * sizeof(int32_t));
     return ok ? VEXB_OK : VEXB_ERR_UNSUPPORTED;
+}
+
+// n values of a per-entry value array to the host in the strip's value type (float-valued strips: widened to double)
+static int download_values(const vexb_spmat *A, void *dst, const void *src, size_t n) {
+    if (!A->val_f32) { VEXB_CUDA(cudaMemcpy(dst, src, n * dtype_size(A->val_dtype), cudaMemcpyDeviceToHost)); return VEXB_OK; }
+    std::vector<float> f(n);
+    VEXB_CUDA(cudaMemcpy(f.data(), src, n * sizeof(float), cudaMemcpyDeviceToHost));
+    std::copy(f.begin(), f.end(), static_cast<double *>(dst));
+    return VEXB_OK;
 }
 
 extern "C" int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, void *ell_val,
@@ -1697,7 +1764,7 @@ extern "C" int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, v
         for (size_t k = 0; k < A->ell_width; ++k)
             for (size_t i = 0; i < A->ell_pitch; ++i)
                 memcpy((char *)ell_val + (i + A->ell_pitch * k) * vs, &ctab[kEllClassHeader + ((size_t)cid[i] * A->ell_width + k) * vs], vs);
-    } else if (ell_val && ne) VEXB_CUDA(cudaMemcpy(ell_val, A->ell_val, ne * vs, cudaMemcpyDeviceToHost));
+    } else if (ell_val && ne) VEXB_TRY(download_values(A, ell_val, A->ell_val, ne));
     if (ell_col && ell_val && ne) {
         // the reference's packing: a row's entries in slots 0, 1, ... (the device layout may leave gaps, see build())
         for (size_t i = 0; i < A->nrows_stored; ++i) {
@@ -1723,7 +1790,7 @@ extern "C" int vexb_spmat_hell_download(const vexb_spmat *A, int32_t *ell_col, v
         } else for (size_t i = 0; i <= A->nrows_stored; ++i) csr_ptr[i] = 0;
     }
     if (csr_col && A->tail_nnz) VEXB_CUDA(cudaMemcpy(csr_col, A->tail_col, A->tail_nnz * 4, cudaMemcpyDeviceToHost));
-    if (csr_val && A->tail_nnz) VEXB_CUDA(cudaMemcpy(csr_val, A->tail_val, A->tail_nnz * vs, cudaMemcpyDeviceToHost));
+    if (csr_val && A->tail_nnz) VEXB_TRY(download_values(A, csr_val, A->tail_val, A->tail_nnz));
     return VEXB_OK;
 }
 
@@ -1733,18 +1800,20 @@ extern "C" int vexb_spmv(int dev, void *stream, const vexb_spmat *A, const void 
     VEXB_CHECK(A->nrows == 0 || y, "y is NULL");
     VEXB_CHECK(A->nnz == 0 || x, "x is NULL");
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
+    if (A->val_dtype == VEXB_F64 && A->val_f32) return spmv_launch<double, float>(A, (cudaStream_t)stream, (const double *)x, (double *)y, alpha, append);
     if (A->val_dtype == VEXB_F64) return spmv_launch<double>(A, (cudaStream_t)stream, (const double *)x, (double *)y, alpha, append);
     return spmv_launch<float>(A, (cudaStream_t)stream, (const float *)x, (float *)y, (float)alpha, append);
 }
 
 // y_k (=|+=) alpha * A x_k for k < nrhs, the matrix streamed once per group of up to 4 right-hand sides (hybrid-ELL
-// strips); other formats, and single vectors, go through vexb_spmv one by one.  vex::SpMat * vex::multivector.
+// strips); other formats, float-valued strips (VEXB_FMT_VALUES_F32) and single vectors go through vexb_spmv one by one.
+// vex::SpMat * vex::multivector.
 extern "C" int vexb_spmv_multi(int dev, void *stream, const vexb_spmat *A, int nrhs, const void *const *x, void *const *y,
                                double alpha, int append) {
     VEXB_CHECK(A && nrhs >= 1 && x && y, "bad arguments");
     VEXB_CHECK(dev == A->dev, "matrix lives on device %d, not %d", A->dev, dev);
     for (int k = 0; k < nrhs; ++k) VEXB_CHECK((A->nrows == 0 || y[k]) && (A->nnz == 0 || x[k]), "vector %d is NULL", k);
-    const bool fused = A->fmt == VEXB_FMT_HELL && A->nnz > 0 && A->nrows_stored > 0 && nrhs > 1 && !param("spmv.no_multi", 0);
+    const bool fused = A->fmt == VEXB_FMT_HELL && !A->val_f32 && A->nnz > 0 && A->nrows_stored > 0 && nrhs > 1 && !param("spmv.no_multi", 0);
     if (!fused) {
         for (int k = 0; k < nrhs; ++k) VEXB_TRY(vexb_spmv(dev, stream, A, x[k], y[k], alpha, append));
         return VEXB_OK;

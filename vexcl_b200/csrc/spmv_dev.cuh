@@ -154,14 +154,16 @@ __device__ __forceinline__ void store_y(T *y, size_t r, T sum, T alpha, int appe
 
 // One row of a hybrid-ELL strip (hybrid_ell.inl:252-268): ELL slots in order, then the CSR tail; products and sums rounded
 // separately.  W > 0: fully unrolled, all 2W streaming loads and then the W gathers of x in flight at once.  Row-class
-// strips: hell_class_rows for one row.
-template <class T, int W, class C>
+// strips: hell_class_rows for one row.  V: stored value type -- T, or float under double vectors (VEXB_FMT_VALUES_F32),
+// widened exactly to T before its product.
+template <class T, int W, class C, class V = T>
 __device__ __forceinline__ T hell_row_sum(size_t i, size_t pitch, int w_dyn, const C *__restrict__ ell_col, const EllShifts &shift,
-                                          const T *__restrict__ ell_val, const int *__restrict__ tail_ptr,
-                                          const int *__restrict__ tail_col, const T *__restrict__ tail_val,
+                                          const V *__restrict__ ell_val, const int *__restrict__ tail_ptr,
+                                          const int *__restrict__ tail_col, const V *__restrict__ tail_val,
                                           const T *__restrict__ x, uint64_t stream, uint64_t keep) {
     static_assert(W > 0 || !std::is_same<C, EllDiag>::value, "the diagonal encoding needs one shift per slot: unrolled widths only");
     if constexpr (std::is_same<C, EllClass>::value) {
+        static_assert(std::is_same<T, V>::value, "row classes keep their table in the vector type");
         const size_t rows[1] = {i};
         T s[1];
         hell_class_rows<T, W, 1>(rows, ell_col, shift, ell_val, tail_ptr, tail_col, tail_val, x, stream, keep, s);
@@ -170,23 +172,23 @@ __device__ __forceinline__ T hell_row_sum(size_t i, size_t pitch, int w_dyn, con
         T sum = T(0);
         const unsigned mask = ell_row_mask(ell_col, i, stream);
         if (W > 0) {
-            int c[W > 0 ? W : 1]; T v[W > 0 ? W : 1]; T xv[W > 0 ? W : 1];
+            int c[W > 0 ? W : 1]; V v[W > 0 ? W : 1]; T xv[W > 0 ? W : 1];
 #pragma unroll
             for (int j = 0; j < W; ++j) { c[j] = ell_slot_column(ell_col, i, pitch, j, ell_shift_of(shift, j), mask, stream); v[j] = ldg_stream(ell_val + i + (size_t)j * pitch, stream); }
 #pragma unroll
             for (int j = 0; j < W; ++j) xv[j] = (c[j] != -1) ? ldg_keep(x + c[j], keep) : T(0);
 #pragma unroll
-            for (int j = 0; j < W; ++j) if (c[j] != -1) sum = t_add<T>(sum, t_mul<T>(v[j], xv[j]));
+            for (int j = 0; j < W; ++j) if (c[j] != -1) sum = t_add<T>(sum, t_mul<T>(T(v[j]), xv[j]));
         } else {
             // any width: plain dependent loop rather than batches of 4 columns: occupancy hides the latency, and a
             // padded slot (column -1) costs 4 bytes, not 12, because its value is never fetched.
             for (int j = 0; j < w_dyn; ++j) {
                 const int c = ell_slot_column(ell_col, i, pitch, j, shift.s[0], mask, stream);   // run-time widths use one shift (spmv.cu build())
-                if (c != -1) sum = t_add<T>(sum, t_mul<T>(ldg_stream(ell_val + i + (size_t)j * pitch, stream), ldg_keep(x + c, keep)));
+                if (c != -1) sum = t_add<T>(sum, t_mul<T>(T(ldg_stream(ell_val + i + (size_t)j * pitch, stream)), ldg_keep(x + c, keep)));
             }
         }
         if (tail_ptr) {
-            for (int j = tail_ptr[i], e = tail_ptr[i + 1]; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(tail_val[j], __ldg(x + tail_col[j])));
+            for (int j = tail_ptr[i], e = tail_ptr[i + 1]; j < e; ++j) sum = t_add<T>(sum, t_mul<T>(T(tail_val[j]), __ldg(x + tail_col[j])));
         }
         return sum;
     }
