@@ -108,8 +108,8 @@ typedef enum {
                              `y = x + A*x` is one launch, y is written once and A*x never goes to memory
                              (vexcl/sparse/product.hpp:45-130, sparse/csr.hpp:102-132, sparse/ell.hpp:207-265,
                              spmat/inline_spmv.hpp:68-76).  Expressions with such terminals run on the NVRTC side path
-                             (the row loop is generated into the kernel, specialised to the strip's format and width);
-                             vexb_reduce does not take them. */
+                             (the row loop is generated into the kernel, specialised to the strip's format and width),
+                             reductions of them included (vexb_reduce_all / vexb_reduce_multi). */
 } vexb_term_kind;
 
 typedef struct {
@@ -244,6 +244,10 @@ int vexb_function_register(const char *name, int ret_dtype, int nargs, const int
 int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile);
 /* The same for the one kernel vexb_eval_multi generates for ncomp (2..8) components. */
 int vexb_jit_source_multi(int lhs_dtype, int assign_op, int ncomp, const vexb_expr *const *exprs, char *buf, size_t *len, int compile);
+/* The same for the kernel that reduces an expression with user functions or inlined sparse products in `dtype`: the one
+ * vexb_reduce_all generates when nops == 1 (ops[0]: any vexb_reduce_op), the one vexb_reduce_multi generates when
+ * nops > 1 (SUM / SUM_KAHAN / MAX / MIN).  The skeleton follows the tunables in force, as at a launch. */
+int vexb_jit_source_reduce(int dtype, int nops, const int *ops, const vexb_expr *expr, char *buf, size_t *len, int compile);
 /* Expressions without a hand-written sweep are served by the pre-compiled interpreter while NVRTC builds a kernel
  * specialised to the expression on a background thread (started at the first use of a new expression shape; tunable
  * "eval.jit": 0 = interpreter only, 1 = compile synchronously, 2 = this, the default).  *pending = 1 while any such
@@ -271,6 +275,10 @@ int vexb_eval_path(int lhs_dtype, int assign_op, const vexb_expr *expr, char *bu
  * (vexb_memset) before first use and is left reusable after each call.
  * Replaces reductor.hpp:327-410; the host fold :412-436 is replaced by
  * vexb_reduce_fetch (single device) or vexb_comm_allreduce (+ fetch).
+ * Expressions that call user functions (VEXB_OP_CALL) or inline sparse products (VEXB_TERM_SPMV) are reduced by ONE
+ * kernel NVRTC generates for the request (compiled at its first use, then cached): the row loop or the call feeds the
+ * fold directly, and the result has the bits of evaluating the expression into a vector of its own type and reducing
+ * that vector with the same tunables.  VEXB_ERR_UNSUPPORTED when NVRTC cannot be loaded: reduce such a temporary then.
  * ---------------------------------------------------------------------- */
 typedef struct vexb_peer vexb_peer;   /* a group of GPUs that write each other's memory; see "Peer memory" below */
 int vexb_reduce_workspace_bytes(int dev, size_t *bytes);

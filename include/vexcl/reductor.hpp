@@ -162,7 +162,8 @@ class Reductor {
                     : vexb_reduce_all(queue[d].ordinal(), queue[d].raw(), &b.e, dt, p.part_size(d), p.part_start(d),
                                       op, res[d].raw(), ws[d].raw(), fused ? ps->peers[d] : nullptr);
                 if (st == VEXB_ERR_UNSUPPORTED && d == 0) {
-                    // the expression calls a user function: evaluate it into a temporary (NVRTC side path), reduce that
+                    // NVRTC cannot be loaded, so the kernel that folds user functions and inlined sparse products in one pass
+                    // cannot be built: evaluate the expression into a temporary, reduce that
                     vex::vector<typename Expr::value_type> tmp(queue, p.size);
                     detail::assign_expression<assign::SET>(tmp, expr, comp);
                     return reduce(tmp, -1);

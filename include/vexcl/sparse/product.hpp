@@ -8,7 +8,8 @@
  * VEXB_TERM_SPMV terminal of the IR, and the expression runs as one NVRTC-generated kernel
  * specialised to the strip's format (CSR, or hybrid ELL with its width unrolled).  `x` may itself
  * be an expression; it is then evaluated into a temporary first (a gather needs all of x).
- * Row-pattern strips and reductions (`sum(f - A*x)`) go through a temporary y instead.
+ * A reduction such as `sum(f - A*x)` is one generated kernel too: the row loop feeds the fold directly.
+ * Row-pattern strips go through a temporary y instead.
  */
 #include <memory>
 #include "../operations.hpp"

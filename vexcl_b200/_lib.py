@@ -130,6 +130,7 @@ def lib():
         "vexb_function_register": ([C.c_char_p, i, i, P(i), C.c_char_p, P(i)], i),
         "vexb_jit_source": ([i, i, P(Expr), C.c_char_p, P(sz), i], i),
         "vexb_jit_source_multi": ([i, i, i, P(P(Expr)), C.c_char_p, P(sz), i], i),
+        "vexb_jit_source_reduce": ([i, i, P(i), P(Expr), C.c_char_p, P(sz), i], i),
         "vexb_reduce_workspace_bytes": ([i, P(sz)], i),
         "vexb_reduce": ([i, vp, P(Expr), i, sz, sz, i, vp, vp], i),
         "vexb_reduce_identity": ([i, vp, i, i, vp], i),

@@ -423,14 +423,30 @@ def _has_call(n) -> bool:
     return any(isinstance(k, Node) and _has_call(k) for k in kids)
 
 
-def _materialize_calls(ctx, expr, n):
-    """Reductions have no run-time compiled form: an expression that calls a user function is first evaluated
-    into a temporary (one extra pass), which is then reduced by the pre-compiled kernel."""
-    if not _has_call(expr):
-        return expr
+def _temporary(ctx, expr, n):
+    """The expression evaluated into a vector of its own type (one extra pass): what a reduction folds when it cannot be
+    served in one kernel."""
     tmp = vector(ctx, n, _VEXB2NP[expr.dtype])
     tmp.assign(expr)
     return tmp
+
+
+def _has_product_temporary(n, part) -> bool:
+    """An inlined product whose strips cannot be inlined (halo, sliced ELL, float values, ...) is evaluated into a
+    temporary product when lowered; a reduction of such an expression keeps the temporary of the whole expression."""
+    if isinstance(n, InlineSpMV):
+        return n.strip(part) is None
+    kids = [getattr(n, c, None) for c in ("a", "b", "cond")] + list(getattr(n, "args", []))
+    return any(isinstance(k, Node) and _has_product_temporary(k, part) for k in kids)
+
+
+def _reduce_in_one_pass(ctx, expr, n):
+    """The expression a Reductor hands to vexb_reduce_all / vexb_reduce_multi.  User functions and inlined sparse
+    products are folded by one kernel generated for the request (bit-identical to reducing their temporary), so the
+    expression goes as it is, unless it holds a product that cannot be inlined."""
+    if _has_call(expr) and _has_product_temporary(expr, ctx.local[0]):
+        return _temporary(ctx, expr, n)
+    return expr
 
 
 def _find_props(n: Node):
@@ -745,8 +761,11 @@ class Reductor:
             ws, r = ctx.workspace(k, K)
             low = _Lowering(k, int(part[k]))
             low.lower(expr)
-            L.check(lib.vexb_reduce_multi(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]), int(part[k]),
-                                          K, ops, r, ws, ctx.peers[k] if fused else None))
+            code = lib.vexb_reduce_multi(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]), int(part[k]),
+                                         K, ops, r, ws, ctx.peers[k] if fused else None)
+            if code == L.ERR_UNSUPPORTED and k == ctx.local[0] and _has_call(expr):
+                return self._combined(_temporary(ctx, expr, n), n, part)       # no NVRTC: reduce a temporary
+            L.check(code)
             res[k] = r
         out = np.empty(K, dtype=self.np_dtype)
         k0 = ctx.local[0]
@@ -778,7 +797,7 @@ class Reductor:
         if props is None:
             raise ValueError("expression has no vector terminal")
         n = props[1]
-        expr = _materialize_calls(ctx, expr, n)
+        expr = _reduce_in_one_pass(ctx, expr, n)
         part = ctx.partition(n)
         if self.kinds is not None:
             return self._combined(expr, n, part)
@@ -789,9 +808,11 @@ class Reductor:
             low = _Lowering(k, int(part[k]))
             low.lower(expr)
             peer = ctx.peers[k] if (ctx.peers is not None and ctx.use_peer_reduce and ctx.nparts > 1) else None
-            _reduce_all_in_step(ctx, k, peer, self.dtype, self.kind, r,
-                                lib.vexb_reduce_all(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]),
-                                                    int(part[k]), self.kind, r, ws, peer), {j: ctx.workspace(j)[1] for j in ctx.local})
+            code = lib.vexb_reduce_all(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]),
+                                       int(part[k]), self.kind, r, ws, peer)
+            if code == L.ERR_UNSUPPORTED and k == ctx.local[0] and _has_call(expr):
+                return self(_temporary(ctx, expr, n))                          # no NVRTC: reduce a temporary
+            _reduce_all_in_step(ctx, k, peer, self.dtype, self.kind, r, code, {j: ctx.workspace(j)[1] for j in ctx.local})
             res[k] = r
         out = np.empty(cnt, dtype=self.np_dtype)
         if ctx.nparts > 1 and ctx.peers is not None and ctx.use_peer_reduce:
@@ -1348,7 +1369,7 @@ def _reduce_device(self, expr, out: DeviceScalar):
         raise ValueError("expression has no vector terminal")
     if self.kind == L.MINMAX:
         raise ValueError("MIN_MAX needs two result slots; use the host-returning call")
-    expr = _materialize_calls(ctx, expr, props[1])
+    expr = _reduce_in_one_pass(ctx, expr, props[1])
     part = ctx.partition(props[1])
     for k in ctx.local:
         ws, _ = ctx.workspace(k)
@@ -1356,9 +1377,11 @@ def _reduce_device(self, expr, out: DeviceScalar):
         low.lower(expr)
         # with a peer group the combine across GPUs happens inside the reduction kernel (no NCCL call)
         peer = ctx.peers[k] if (ctx.peers is not None and ctx.use_peer_reduce) else None
-        _reduce_all_in_step(ctx, k, peer, self.dtype, self.kind, out.bufs[k],
-                            lib.vexb_reduce_all(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]),
-                                                int(part[k]), self.kind, out.bufs[k], ws, peer), out.bufs)
+        code = lib.vexb_reduce_all(ctx.devs[k], ctx.streams[k], C.byref(low.e), self.dtype, int(part[k + 1] - part[k]),
+                                   int(part[k]), self.kind, out.bufs[k], ws, peer)
+        if code == L.ERR_UNSUPPORTED and k == ctx.local[0] and _has_call(expr):
+            return _reduce_device(self, _temporary(ctx, expr, props[1]), out)   # no NVRTC: reduce a temporary
+        _reduce_all_in_step(ctx, k, peer, self.dtype, self.kind, out.bufs[k], code, out.bufs)
     if ctx.nparts > 1 and not (ctx.peers is not None and ctx.use_peer_reduce):
         if ctx.comms is None:
             raise RuntimeError("device-resident reductions over several slots need a communicator (NCCL)")

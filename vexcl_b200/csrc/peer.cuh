@@ -1,105 +1,11 @@
-// One-hop all-reduce over NVLink peer memory, callable from inside a kernel.
-//
-// Every rank owns a small "mailbox" in device memory that all other ranks can write (CUDA IPC mapping
-// between processes, peer access inside one process).  To combine one value per rank:
-//     each rank stores its value into slot[parity][my_rank] of EVERY rank's mailbox (plain stores over
-//     NVLink), fences, and publishes flag[parity][my_rank] = epoch with a system-scope release store;
-//     then it waits (acquire loads) until its own mailbox holds flags >= epoch from all ranks and folds the
-//     nranks values in rank order -- the same order on every rank, so all ranks get bit-identical results.
-// The epoch lives in the mailbox and is advanced by the kernel itself, so a captured CUDA graph can be
-// replayed.  Slots are double-buffered by epoch parity: a rank can only be one all-reduce ahead of the
-// slowest rank (finishing epoch e needs everybody's contribution to e), so parity e+2 never overwrites
-// values somebody still has to read.
-//
-// This is what the last block of the reduction kernel runs (csrc/reduce.cu), which makes
-// "reduce the slice + combine across GPUs" ONE kernel with no NCCL call and no host involvement; it
-// replaces the host fold of vexcl/reductor.hpp:412-436.
+// One-hop all-reduce over NVLink peer memory, callable from inside a kernel: the protocol and its device side
+// (PeerArgs, peer_exchange, peer_poison) live in fold.cuh, next to the reduction finish that calls them, because the
+// NVRTC-generated reductions embed that text too.  This header adds the host side: the group handle vexb_peer.
 #pragma once
 #include "common.cuh"
-
-#define VEXB_MAX_PEERS 16
+#include "fold.cuh"
 
 namespace vexb {
-
-struct PeerArgs {
-    unsigned long long *mbox[VEXB_MAX_PEERS];   // mbox[p]: rank p's mailbox as seen from this rank
-    int rank, nranks;                           // nranks == 0: disabled
-    unsigned long long *fault_host;             // process-wide sticky fault word (mapped pinned host memory), may be NULL
-};
-
-// mailbox layout in 8-byte words: [0] epoch, [1] error flag, [16 + ((parity*nranks + src) * 4) + {0,1,2}] = value0, value1, flag
-__device__ __forceinline__ unsigned long long *peer_slot(unsigned long long *mbox, int parity, int nranks, int src) {
-    return mbox + 16 + (size_t)(parity * nranks + src) * 4;
-}
-
-__device__ __forceinline__ void st_release_sys(unsigned long long *p, unsigned long long v) {
-    asm volatile("st.release.sys.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long *p) {
-    unsigned long long v;
-    asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ unsigned long long ld_relaxed_sys(const unsigned long long *p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-
-// Called by ALL threads of one block (blockDim.x >= nranks).  v0/v1: this rank's contribution as raw 64-bit
-// words (thread 0's arguments are used).  On return out0[s]/out1[s] (shared memory, s < nranks) hold every
-// rank's words; the caller folds them in rank order.  Returns false (to every thread) when a peer did not arrive
-// within ~20 s: the slots are then NOT valid and the caller must not fold them -- it stores NaN / the all-ones
-// pattern instead and the fault is made sticky (mailbox word 1 and the process-wide fault word, vexb_peer_fault),
-// so that vexb_reduce_fetch and the front ends fail loudly instead of returning a wrong sum.
-__device__ __forceinline__ bool peer_exchange(const PeerArgs &pa, unsigned long long v0, unsigned long long v1,
-                                              unsigned long long *out0, unsigned long long *out1) {
-    __shared__ unsigned long long sh[3];
-    __shared__ int sh_ok;
-    unsigned long long *mine = pa.mbox[pa.rank];
-    if (threadIdx.x == 0) {
-        const unsigned long long e = mine[0] + 1;
-        mine[0] = e;
-        sh[0] = e; sh[1] = v0; sh[2] = v1; sh_ok = 1;
-    }
-    __syncthreads();
-    const unsigned long long e = sh[0];
-    const int parity = (int)(e & 1ull);
-    if ((int)threadIdx.x < pa.nranks) {
-        // push my contribution into rank `threadIdx.x`'s mailbox
-        unsigned long long *dst = peer_slot(pa.mbox[threadIdx.x], parity, pa.nranks, pa.rank);
-        dst[0] = sh[1]; dst[1] = sh[2];
-        __threadfence_system();
-        st_release_sys(dst + 2, e);
-        // collect rank `threadIdx.x`'s contribution from my own mailbox
-        const unsigned long long *src = peer_slot(mine, parity, pa.nranks, threadIdx.x);
-        bool ok = ld_acquire_sys(src + 2) >= e;
-        if (!ok) {
-            unsigned long long t0; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t0));
-            for (unsigned it = 0; !ok; ++it) {
-                ok = ld_acquire_sys(src + 2) >= e;
-                if (ok) break;
-                __nanosleep(it < 64 ? 20 : 200);
-                if ((it & 1023u) == 1023u) {
-                    unsigned long long t1; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t1));
-                    if (t1 - t0 > 20000000000ull) break;
-                }
-            }
-        }
-        if (!ok) {                                  // peer never arrived: sticky fault, nothing is folded
-            mine[1] = e;
-            if (pa.fault_host) *pa.fault_host = e;
-            atomicExch(&sh_ok, 0);
-        }
-        out0[threadIdx.x] = ok ? ld_relaxed_sys(src) : 0ull;
-        out1[threadIdx.x] = ok ? ld_relaxed_sys(src + 1) : 0ull;
-    }
-    __syncthreads();
-    return sh_ok != 0;
-}
-
-// What a result holds after a failed exchange: NaN for floating types, all ones for integers.
-template <class T> __device__ __forceinline__ T peer_poison() { T v; memset(&v, 0xff, sizeof(T)); return v; }
 
 // Process-wide sticky fault word in mapped pinned host memory (peer.cu): 0 = no fault.
 unsigned long long *peer_fault_word();

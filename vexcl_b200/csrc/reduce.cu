@@ -11,127 +11,12 @@
 // for vexb_comm_allreduce or a single 8-byte D2H.
 #include "expr_eval.cuh"
 #include "shapes.cuh"
-#include "peer.cuh"
-#include <limits>
+#include "peer.cuh"      // fold.cuh: Fold, RtFold, block_finish, the peer exchange
 
 namespace vexb {
 
-template <class T> struct Lim {
-    static __host__ __device__ T lowest() { return std::numeric_limits<T>::lowest(); }
-    static __host__ __device__ T highest() { return std::numeric_limits<T>::max(); }
-};
-
-template <class T> __device__ __forceinline__ T red_add(T a, T b) { return a + b; }
-template <> __device__ __forceinline__ double red_add<double>(double a, double b) { return __dadd_rn(a, b); }
-template <> __device__ __forceinline__ float red_add<float>(float a, float b) { return __fadd_rn(a, b); }
-template <class T> __device__ __forceinline__ T red_sub(T a, T b) { return a - b; }
-template <> __device__ __forceinline__ double red_sub<double>(double a, double b) { return __dsub_rn(a, b); }
-template <> __device__ __forceinline__ float red_sub<float>(float a, float b) { return __fsub_rn(a, b); }
-
-// Fold state: x (and y for Kahan's compensation / MINMAX's max).
-template <int OP, class T> struct Fold {
-    T x, y;
-    __device__ __forceinline__ void init() {
-        if (OP == VEXB_SUM || OP == VEXB_SUM_KAHAN) { x = T(0); y = T(0); }
-        else if (OP == VEXB_MAX) { x = Lim<T>::lowest(); y = T(0); }
-        else if (OP == VEXB_MIN) { x = Lim<T>::highest(); y = T(0); }
-        else { x = Lim<T>::highest(); y = Lim<T>::lowest(); }
-    }
-    // Same statement order as the reference's per-work-item loops
-    // (reductor.hpp:511-533 plain, :537-564 Kahan; ops :60-63, :92-95, :116-119).
-    __device__ __forceinline__ void take(T v) {
-        if (OP == VEXB_SUM) x = red_add<T>(x, v);
-        else if (OP == VEXB_SUM_KAHAN) { const T yy = red_sub<T>(v, y); const T t = red_add<T>(x, yy); y = red_sub<T>(red_sub<T>(t, x), yy); x = t; }
-        else if (OP == VEXB_MAX) x = x > v ? x : v;
-        else if (OP == VEXB_MIN) x = x < v ? x : v;
-        else { x = x < v ? x : v; y = y > v ? y : v; }
-    }
-    __device__ __forceinline__ void merge(const Fold &o) {
-        if (OP == VEXB_SUM || OP == VEXB_SUM_KAHAN) x = red_add<T>(x, o.x);   // tree/host stages are plain adds in the reference too
-        else if (OP == VEXB_MAX) x = x > o.x ? x : o.x;
-        else if (OP == VEXB_MIN) x = x < o.x ? x : o.x;
-        else { x = x < o.x ? x : o.x; y = y > o.y ? y : o.y; }
-    }
-};
-
-template <int OP, class T>
-__device__ __forceinline__ Fold<OP, T> shfl_down_fold(const Fold<OP, T> &f, int off) {
-    Fold<OP, T> r;
-    r.x = __shfl_down_sync(0xffffffffu, f.x, off);
-    r.y = (OP == VEXB_MINMAX) ? __shfl_down_sync(0xffffffffu, f.y, off) : T(0);
-    return r;
-}
-
-struct ReduceWs {               // layout of d_workspace
-    unsigned int ticket;        // zero between calls
-    unsigned int pad[15];
-    // followed by 2 * max_blocks values of 8 bytes
-};
-
-template <class T> __device__ __forceinline__ unsigned long long to_bits(T v) { unsigned long long u = 0; memcpy(&u, &v, sizeof(T)); return u; }
-template <class T> __device__ __forceinline__ T from_bits(unsigned long long u) { T v; memcpy(&v, &u, sizeof(T)); return v; }
-
-template <int OP, class T>
-__device__ __forceinline__ void block_finish(Fold<OP, T> f, void *ws, T *result, const PeerArgs &pa) {
-    __shared__ T sx[8], sy[8];
-    __shared__ bool is_last;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) f.merge(shfl_down_fold<OP, T>(f, off));
-    if (lane == 0) { sx[warp] = f.x; sy[warp] = f.y; }
-    __syncthreads();
-    T *partials = reinterpret_cast<T *>(reinterpret_cast<char *>(ws) + sizeof(ReduceWs));
-    unsigned int *ticket = &reinterpret_cast<ReduceWs *>(ws)->ticket;
-    if (threadIdx.x == 0) {
-        Fold<OP, T> b; b.x = sx[0]; b.y = sy[0];
-        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) { Fold<OP, T> o; o.x = sx[w]; o.y = sy[w]; b.merge(o); }
-        partials[2 * blockIdx.x] = b.x; partials[2 * blockIdx.x + 1] = b.y;
-        __threadfence();
-        const unsigned int t = atomicAdd(ticket, 1u);
-        is_last = (t == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    // last block: fold partials[0..gridDim.x) in a fixed order
-    Fold<OP, T> g; g.init();
-    if (OP == VEXB_SUM_KAHAN) { /* plain adds from here on */ }
-    for (unsigned int b = threadIdx.x; b < gridDim.x; b += blockDim.x) {
-        Fold<OP, T> o;
-        o.x = __ldcg(&partials[2 * b]); o.y = __ldcg(&partials[2 * b + 1]);
-        g.merge(o);
-    }
-    if (OP == VEXB_SUM_KAHAN) g.y = T(0);
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) g.merge(shfl_down_fold<OP, T>(g, off));
-    __syncthreads();
-    if (lane == 0) { sx[warp] = g.x; sy[warp] = g.y; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        Fold<OP, T> b; b.x = sx[0]; b.y = sy[0];
-        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) { Fold<OP, T> o; o.x = sx[w]; o.y = sy[w]; b.merge(o); }
-        sx[0] = b.x; sy[0] = b.y;
-        *ticket = 0;
-    }
-    __syncthreads();
-    if (pa.nranks > 1) {
-        // combine across GPUs in the same kernel: one-hop exchange over NVLink peer memory (peer.cuh)
-        __shared__ unsigned long long px[VEXB_MAX_PEERS], py[VEXB_MAX_PEERS];
-        const bool arrived = peer_exchange(pa, to_bits<T>(sx[0]), to_bits<T>(sy[0]), px, py);
-        if (threadIdx.x == 0) {
-            if (arrived) {
-                Fold<OP, T> b; b.x = from_bits<T>(px[0]); b.y = from_bits<T>(py[0]);
-                for (int r = 1; r < pa.nranks; ++r) { Fold<OP, T> o; o.x = from_bits<T>(px[r]); o.y = from_bits<T>(py[r]); b.merge(o); }
-                sx[0] = b.x; sy[0] = b.y;
-            } else { sx[0] = peer_poison<T>(); sy[0] = peer_poison<T>(); }   // a peer timed out: never a partial fold (peer.cuh)
-        }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        result[0] = sx[0];
-        if (OP == VEXB_MINMAX) result[1] = sy[0];
-    }
-}
+int jit_reduce(int dev, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t index_offset, int nops, const int *ops,
+               bool multi, size_t cap, void *d_result, void *d_workspace, const PeerArgs &pa);
 
 template <int SH, int OP, class T, int U>
 __global__ void __launch_bounds__(256) reduce_sweep_kernel(SweepArgs a, size_t n, void *ws, T *result, PeerArgs pa) {
@@ -312,27 +197,9 @@ __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constan
 }
 
 // ---- several reductions of ONE expression in one pass: vex::CombineReductors<R...> (reductor.hpp:132-280) ------------
-// The expression is evaluated once per element and fed to up to VEXB_MAX_COMBINED folds; every fold then finishes like a
-// single reduction (its own partials and ticket in its own slice of the workspace, its own combine across the GPUs).
-template <class T>
-struct RtFold {
-    T x, y;
-    __device__ __forceinline__ void init(int op) {
-        x = (op == VEXB_MAX) ? Lim<T>::lowest() : (op == VEXB_MIN) ? Lim<T>::highest() : T(0); y = T(0);
-    }
-    __device__ __forceinline__ void take(int op, T v) {
-        if (op == VEXB_SUM) x = red_add<T>(x, v);
-        else if (op == VEXB_SUM_KAHAN) { const T yy = red_sub<T>(v, y); const T t = red_add<T>(x, yy); y = red_sub<T>(red_sub<T>(t, x), yy); x = t; }
-        else if (op == VEXB_MAX) x = x > v ? x : v;
-        else x = x < v ? x : v;
-    }
-    __device__ __forceinline__ void merge(int op, const RtFold &o) {
-        if (op == VEXB_SUM || op == VEXB_SUM_KAHAN) x = red_add<T>(x, o.x);
-        else if (op == VEXB_MAX) x = x > o.x ? x : o.x;
-        else x = x < o.x ? x : o.x;
-    }
-};
-
+// The expression is evaluated once per element and fed to up to VEXB_MAX_COMBINED folds (RtFold, fold.cuh); every fold then
+// finishes like a single reduction (its own partials and ticket in its own slice of the workspace, its own combine across
+// the GPUs).
 struct MultiOps { int n; int op[VEXB_MAX_COMBINED]; };
 
 template <class T, int U>
@@ -456,9 +323,6 @@ extern "C" int vexb_reduce_all(int dev, void *stream, const vexb_expr *expr, int
     if (op == VEXB_SUM_KAHAN && !dtype_is_float(dtype)) op = VEXB_SUM;
     vexb_expr e;
     VEXB_TRY(normalize_expr(expr, &e, n != 0));
-    if (expr_has_call(e) || expr_has_spmv(e))
-        VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "reductions of expressions that call user functions or inline a sparse product are evaluated into a "
-                                        "temporary first (the front ends do this); vexb_reduce itself has no run-time compiled form");
     if (n == 0) {                                                               // reductor.hpp:318-321
         VEXB_TRY(vexb_reduce_identity(dev, stream, dtype, op, d_result));
         return pa.nranks > 1 ? vexb_peer_allreduce(peer, stream, d_result, dtype, op) : VEXB_OK;
@@ -469,6 +333,8 @@ extern "C" int vexb_reduce_all(int dev, void *stream, const vexb_expr *expr, int
     long bps = param("reduce.blocks_per_sm", 8);
     if (bps < 1) bps = 1; if (bps > kMaxBlocksPerSm) bps = kMaxBlocksPerSm;
     const size_t cap = (size_t)sms * (size_t)bps;
+    // user functions and inlined sparse products have no pre-compiled form: one kernel generated for the request (jit.cu)
+    if (expr_has_call(e) || expr_has_spmv(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, 1, &op, false, cap, d_result, d_workspace, pa);
 
     if ((dtype == VEXB_F64 || dtype == VEXB_F32) && !param("eval.force_interp", 0)) {
         ShapeMatch m = match_shape(e, dtype);
@@ -577,7 +443,6 @@ extern "C" int vexb_reduce_multi(int dev, void *stream, const vexb_expr *expr, i
     if (peer && peer->nranks > 1) { VEXB_CHECK(peer->dev == dev, "peer group lives on device %d, not %d", peer->dev, dev); pa = peer->args(); }
     vexb_expr e;
     VEXB_TRY(normalize_expr(expr, &e, n != 0));
-    if (expr_has_call(e) || expr_has_spmv(e)) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "reductions of expressions that call user functions or inline a sparse product are evaluated into a temporary first");
     const size_t es = dtype_size(dtype);
     if (n == 0) {
         for (int k = 0; k < nops; ++k) {
@@ -595,6 +460,7 @@ extern "C" int vexb_reduce_multi(int dev, void *stream, const vexb_expr *expr, i
     size_t want = (n + 1023) / 1024;
     const int blocks = (int)(want < cap ? want : cap);
     cudaStream_t st = (cudaStream_t)stream;
+    if (expr_has_call(e) || expr_has_spmv(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, nops, mo.op, true, cap, d_result, d_workspace, pa);
     switch (dtype) {
         case VEXB_F64: launch_rmulti<double>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
         case VEXB_F32: launch_rmulti<float>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
