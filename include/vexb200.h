@@ -28,6 +28,10 @@
  *   vexb_zsr_create /
  *   vexb_zspmv          <- sparse::matrix<std::complex<T>> ctor + product with
  *                          the spmv_ops_impl of examples/complex_spmv.cpp
+ *   vexb_usr_create /
+ *   vexb_usr_spmv       <- sparse::matrix<user value type> ctor + product
+ *                          generated from its spmv_ops_impl snippets
+ *                          (sparse/spmv_ops.hpp, sparse/csr.hpp:109-126)
  *   vexb_dspmat_*       <- SpMat ctor + SpMat::apply (vexcl/spmat.hpp:71-185)
  *   vexb_ccsr_*         <- SpMatCCSR ctor + its generated product function
  *                          (vexcl/spmat/ccsr.hpp:70-78, :176-201)
@@ -514,6 +518,53 @@ int vexb_zspmat_destroy(vexb_zspmat *A);
 int vexb_zspmat_get_info(const vexb_zspmat *A, vexb_zspmat_info *info);
 /* y (=|+=) alpha * A x, alpha real; with no stored entry, y = A*x zeroes y and y += A*x leaves it as it is. */
 int vexb_zspmv(int dev, void *stream, const vexb_zspmat *A, const void *x, void *y, double alpha, int append);
+
+/* ------------------------------------------------------------------------
+ * Sparse strips of user value types (one device): vex::sparse::{csr, ell,
+ * matrix}<V> for a type V the user declares with vex::is_cl_native,
+ * vex::type_name_impl, vex::sparse::rhs_of and vex::sparse::spmv_ops_impl
+ * (the reference's sparse/spmv_ops.hpp).  The library does not know the
+ * components of V: each value is val_bytes opaque bytes, stored as the
+ * complex strips above with one component of val_bytes per slot (lane l of
+ * slot k in slice s holds value slice_ptr[s] + 32k + l; padding is zero).
+ * The product kernel is generated from the snippets of vexb_usr_ops and
+ * compiled by NVRTC for sm_90a (--fmad=false) at its first use on a device,
+ * then cached.  For each row, in storage order:
+ *   decl;  append_product(sum, v, xv) for every stored value v, xv = x[col];
+ *   then y_r = sum (append = 0)  or  t = y_r; append(t, sum); y_r = t.
+ * There is no alpha: spmv_ops_impl has no hook for scaling or negation.
+ * create() validates every argument before it touches a device.
+ * ---------------------------------------------------------------------- */
+typedef struct vexb_usrmat vexb_usrmat;
+typedef struct {
+    size_t  nrows, ncols, nnz;       /* rows, columns, stored values */
+    int32_t val_bytes;               /* sizeof(V) */
+    size_t  n_slices, n_slots;       /* sliced-ELL slices of 32 rows, slots over all slices (as vexb_csr_sell_layout) */
+    size_t  device_bytes;            /* n_slots * (val_bytes + 4) + perm + slice_ptr */
+} vexb_usrmat_info;
+/* The device side of spmv_ops_impl<V, X>.  Snippets use the fixed names sum (the accumulator, declared by decl),
+ * v (const V, the stored value), xv (const X, x at its column) and t (X, the old y_r).  The generated source holds
+ * static_assert(sizeof(V) == val_bytes && sizeof(X) == rhs_bytes), so a host/device size mismatch fails in NVRTC. */
+typedef struct {
+    const char *val_type;            /* device type name of V, e.g. "double4" */
+    const char *rhs_type;            /* device type name of X, the element of x and y, e.g. "double2" */
+    size_t      rhs_bytes;           /* sizeof(X) on the host, 1..64 */
+    const char *decl;                /* spmv_ops_impl<V, X>::decl_accum_var(src, "sum") */
+    const char *product;             /* spmv_ops_impl<V, X>::append_product(src, "sum", "v", "xv") */
+    const char *append;              /* spmv_ops_impl<V, X>::append(src, "t", "sum") */
+} vexb_usr_ops;
+/* val: nnz values of val_bytes bytes each (val_bytes a multiple of 4 in 4..64), the bytes of V[nnz]. */
+int vexb_usr_create(int dev, void *stream, size_t nrows, size_t ncols, const void *ptr, int ptr_bytes,
+                    const void *col, int col_bytes, const void *val, int val_bytes, vexb_usrmat **out);
+int vexb_usrmat_destroy(vexb_usrmat *A);
+int vexb_usrmat_get_info(const vexb_usrmat *A, vexb_usrmat_info *info);
+/* y (=|+=) A x with x: ncols X and y: nrows X, both aligned to the natural alignment of an X of rhs_bytes (the largest
+ * power of two up to 16 that divides it).  With no stored value, y = A*x zeroes y and y += A*x leaves it as it is.  An
+ * NVRTC failure returns VEXB_ERR_INVALID with the compiler's log in vexb_last_error(). */
+int vexb_usr_spmv(int dev, void *stream, const vexb_usrmat *A, const vexb_usr_ops *ops, const void *x, void *y, int append);
+/* Source of the kernel vexb_usr_spmv generates for these ops (compile != 0: also compiled by NVRTC for sm_90a, no device
+ * needed).  *len in: capacity, out: bytes needed. */
+int vexb_jit_source_usr(const vexb_usr_ops *ops, int val_bytes, char *buf, size_t *len, int compile);
 
 /* ------------------------------------------------------------------------
  * Compressed CSR for stencil-like matrices: vex::SpMatCCSR

@@ -8,9 +8,10 @@
  *   is_cpu, queue_list            (vexcl/backend/cuda/context.hpp:96-413,
  *                                  vexcl/backend/cuda/device_vector.hpp:42-210,
  *                                  vexcl/backend/cuda/error.hpp:49-160)
- * There is no source_generator / kernel / build_sources here: kernels are
- * pre-compiled sm_90a code inside the library, selected at run time from an
- * expression IR (see operations.hpp).
+ * There is no kernel / build_sources here: kernels are pre-compiled sm_90a
+ * code inside the library, selected at run time from an expression IR (see
+ * operations.hpp).  source_generator is reduced to what the snippets of a
+ * user's vex::sparse::spmv_ops_impl need (sparse/spmv_ops.hpp).
  */
 #include <cstddef>
 #include <cstdint>
@@ -285,6 +286,22 @@ std::vector<device> device_list(DevFilter &&filter) {
     for (int d = 0; d < n; ++d) if (f(device(d))) out.push_back(device(d));
     return out;
 }
+
+/// The part of the reference's source generator (vexcl/backend/cuda/source.hpp) that vex::sparse::spmv_ops_impl bodies
+/// use: they write the device snippets of a user value type's sparse product (sparse/spmv_ops.hpp).  Numbers are written
+/// with enough digits to read back the same double.
+class source_generator {
+    public:
+        source_generator() { src.precision(17); }
+        source_generator& new_line() { src << "\n" << std::string(2 * indent, ' '); return *this; }
+        source_generator& open(const char *bracket) { new_line() << bracket; ++indent; return *this; }
+        source_generator& close(const char *bracket) { if (indent) --indent; new_line() << bracket; return *this; }
+        template <class T> source_generator& operator<<(const T &v) { src << v; return *this; }
+        std::string str() const { return src.str(); }
+    private:
+        std::ostringstream src;
+        unsigned indent = 2;            // the snippets go into the body of a loop of the generated kernel
+};
 
 } // namespace backend
 } // namespace vex

@@ -307,16 +307,26 @@ struct additive_operator {
     void apply(V &y, typename V::value_type sign, bool append) const { A.apply(x, y, sign * scale, append); }
 };
 
-/// `M * x` that M writes straight into y with one call, M::mul(x, y, alpha, append): the product of a block or complex
-/// sparse matrix (sparse/matrix.hpp).  vex::vector takes it as y = A*x, y += A*x and y -= A*x.  It has no kernel form, so any other
-/// expression that holds it stops at the static_assert below.
+namespace detail {
+/// The scalar of a direct product's vector element: T of std::array<T, B> and std::complex<T>.  A user value type has none;
+/// double stands in for it, so that expression nodes around a misused product still form and stop at a static_assert.
+template <class R, class = void> struct direct_scalar { typedef double type; };
+template <class R> struct direct_scalar<R, decltype(void(std::declval<typename R::value_type>()))> { typedef typename R::value_type type; };
+/// Can M::mul scale its product (alpha != 1)?  Not when M says `static const bool scales = false` (user value types).
+template <class M, class = void> struct direct_scales : std::true_type {};
+template <class M> struct direct_scales<M, typename std::enable_if<!M::scales>::type> : std::false_type {};
+}
+
+/// `M * x` that M writes straight into y with one call, M::mul(x, y, alpha, append): the product of a block, complex or
+/// user-value sparse matrix (sparse/matrix.hpp).  vex::vector takes it as y = A*x, y += A*x and, unless M is of a user
+/// value type, y -= A*x.  It has no kernel form, so any other expression that holds it stops at the static_assert below.
 template <class M, class V>
 struct direct_product : vector_expr_tag {
     static const bool hold_by_reference = false;
-    typedef typename M::rhs_type::value_type value_type;   // the block's or complex's scalar: expression nodes around a misused product still form
+    typedef typename detail::direct_scalar<typename M::rhs_type>::type value_type;   // expression nodes around a misused product still form
     const M &A; const V &x;
     direct_product(const M &A, const V &x) : A(A), x(x) {}
-    void props(detail::expr_props&) const { static_assert(sizeof(M) == 0, "a block or complex matrix product is only assigned: Y = A * X, Y += A * X or Y -= A * X"); }
+    void props(detail::expr_props&) const { static_assert(sizeof(M) == 0, "a block, complex or user-value matrix product is only assigned: Y = A * X, Y += A * X or (not for user value types) Y -= A * X"); }
     int lower(detail::ir_builder&) const { return -1; }
 };
 

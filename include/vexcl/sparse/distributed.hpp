@@ -28,6 +28,8 @@ class distributed {
                       "vex::sparse::distributed does not take block values: use vex::sparse::matrix on a single device");
         static_assert(!detail_sparse::is_complex_value<value_type>::value,
                       "vex::sparse::distributed does not take complex values: use vex::sparse::matrix on a single device");
+        static_assert(!detail_sparse::is_user_value<value_type>::value,
+                      "vex::sparse::distributed does not take user value types: use vex::sparse::matrix on a single device");
 
         template <class PtrRange, class ColRange, class ValRange>
         distributed(const std::vector<backend::command_queue> &q, size_t nrows, size_t ncols,

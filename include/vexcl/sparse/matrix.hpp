@@ -6,8 +6,9 @@
  * csr -> the TMA-staged CSR row-block kernel, ell -> hybrid ELL (the reference's layout and width
  * rule; its device-side csr2ell conversion, ell.hpp:348-506, happens on the host at upload here),
  * matrix -> libvexb200's own choice (the reference picks csr on CPUs and ell on GPUs).
- * With B x B block values (std::array<std::array<T, B>, B>) all three are the block format below, and with
- * std::complex<T> values the complex format below.
+ * With B x B block values (std::array<std::array<T, B>, B>) all three are the block format below, with
+ * std::complex<T> values the complex format below, and with a user value type (vex::is_user_value, a product given
+ * by its vex::sparse::spmv_ops_impl) the user-value format below.
  */
 #include <array>
 #include <complex>
@@ -15,6 +16,7 @@
 #include <memory>
 #include "../vector.hpp"
 #include "product.hpp"
+#include "spmv_ops.hpp"
 
 namespace vex {
 namespace sparse {
@@ -24,7 +26,7 @@ template <class R> inline size_t range_size(const R &r) { return static_cast<siz
 template <class R> inline auto range_data(const R &r) -> decltype(&*std::begin(r)) { return range_size(r) ? &*std::begin(r) : nullptr; }
 }
 
-template <int Format, typename Val, typename Col, typename Ptr>
+template <int Format, typename Val, typename Col, typename Ptr, typename Enable = void>
 class single_device_matrix {
     public:
         typedef Val value_type; typedef Val val_type; typedef Col col_type; typedef Ptr ptr_type;
@@ -144,6 +146,8 @@ class single_device_matrix<Format, std::array<std::array<T, B>, B>, Col, Ptr> {
 namespace detail_sparse {
 template <class V> struct is_complex_value : std::false_type {};
 template <class T> struct is_complex_value<std::complex<T>> : std::true_type {};
+template <class V> struct is_user_value
+    : std::integral_constant<bool, vex::is_user_value<V>::value && !is_block_value<V>::value && !is_complex_value<V>::value> {};
 }
 
 /// Complex matrices: std::complex<double> or std::complex<float> values, the reference's examples/complex_spmv.cpp.  x and
@@ -199,6 +203,77 @@ class single_device_matrix<Format, std::complex<T>, Col, Ptr> {
         std::vector<backend::command_queue> q;
         size_t n, m, nnz;
         std::shared_ptr<vexb_zspmat> A;
+};
+
+/// Matrices of a user value type V (vex::is_user_value: is_cl_native<V> specialised true, V neither arithmetic, nor a
+/// block, nor complex), the reference's sparse/spmv_ops.hpp: x and y are vex::vector<rhs_of<V>::type>, and the product is
+/// generated from spmv_ops_impl<V, rhs_of<V>::type>, whose snippets are built once, here, and compiled by NVRTC at the
+/// first product on a device.  csr, ell and matrix all take the one user-value format of libvexb200 (sliced ELL,
+/// vexb_usr_create).  `Y = A * X` and `Y += A * X` are one vexb_usr_spmv launch into Y.  spmv_ops_impl has no hook for
+/// negation or scaling, so `Y -= A * X` and scaled products stop at a static_assert, and the product takes part in no
+/// other expression.
+template <int Format, typename V, typename Col, typename Ptr>
+class single_device_matrix<Format, V, Col, Ptr, typename std::enable_if<detail_sparse::is_user_value<V>::value>::type> {
+    public:
+        typedef V value_type; typedef value_type val_type; typedef Col col_type; typedef Ptr ptr_type;
+        typedef typename rhs_of<value_type>::type rhs_type;
+        static const bool scales = false;           // direct_product: no Y -= A * X
+        static_assert(sizeof(V) % 4 == 0 && sizeof(V) <= 64, "a user value type must be a multiple of 4 bytes, at most 64");
+
+        template <class PtrRange, class ColRange, class ValRange>
+        single_device_matrix(const std::vector<backend::command_queue> &q, size_t nrows, size_t ncols,
+                             const PtrRange &ptr, const ColRange &col, const ValRange &val, bool /*fast_setup*/ = true)
+            : q(q), n(nrows), m(ncols), nnz(detail_sparse::range_size(val))
+        {
+            precondition(q.size() == 1, "sparse matrices of this kind are only supported for single-device contexts");
+            static_assert(sizeof(Col) == 4 || sizeof(Col) == 8, "column type must be 32 or 64 bit");
+            static_assert(sizeof(Ptr) == 4 || sizeof(Ptr) == 8, "pointer type must be 32 or 64 bit");
+            typedef spmv_ops_impl<value_type, rhs_type> ops;
+            backend::source_generator d, p, a;
+            ops::decl_accum_var(d, "sum");
+            ops::append_product(p, "sum", "v", "xv");
+            ops::append(a, "t", "sum");
+            src = std::make_shared<std::array<std::string, 5>>(std::array<std::string, 5>{
+                {type_name<value_type>(), type_name<rhs_type>(), d.str(), p.str(), a.str()}});
+            vexb_usrmat *h = nullptr;
+            VEXB_CHECKED(vexb_usr_create(q[0].ordinal(), q[0].raw(), nrows, ncols, detail_sparse::range_data(ptr), sizeof(Ptr),
+                                         detail_sparse::range_data(col), sizeof(Col), detail_sparse::range_data(val),
+                                         static_cast<int>(sizeof(value_type)), &h));
+            A.reset(h, [](vexb_usrmat *p) { vexb_usrmat_destroy(p); });
+        }
+        single_device_matrix() : n(0), m(0), nnz(0) {}
+
+        size_t rows() const { return n; }
+        size_t cols() const { return m; }
+        size_t nonzeros() const { return nnz; }
+        const std::vector<backend::command_queue>& queue_list() const { return q; }
+
+        /// y = A * x   or   y += A * x; alpha must be 1 (Y -= A * X does not compile)
+        void mul(const vex::vector<rhs_type> &x, vex::vector<rhs_type> &y, double alpha = 1, bool append = false) const {
+            precondition(alpha == 1, "a product of a user value type is not scaled");
+            precondition(x.size() == m && y.size() == n, "sparse product: vector sizes do not match the matrix");
+            const std::array<std::string, 5> &s = *src;
+            vexb_usr_ops o;
+            o.val_type = s[0].c_str(); o.rhs_type = s[1].c_str(); o.rhs_bytes = sizeof(rhs_type);
+            o.decl = s[2].c_str(); o.product = s[3].c_str(); o.append = s[4].c_str();
+            VEXB_CHECKED(vexb_usr_spmv(q[0].ordinal(), q[0].raw(), A.get(), &o, x(0).raw(), y(0).raw(), append));
+        }
+
+        friend direct_product<single_device_matrix, vex::vector<rhs_type>> operator*(const single_device_matrix &A, const vex::vector<rhs_type> &x) {
+            return direct_product<single_device_matrix, vex::vector<rhs_type>>(A, x);
+        }
+        template <class Expr>
+        friend typename std::enable_if<is_vector_expr<Expr>::value && !std::is_same<Expr, vex::vector<rhs_type>>::value,
+                                       direct_product<single_device_matrix, Expr>>::type
+        operator*(const single_device_matrix &A, const Expr &x) {
+            static_assert(sizeof(Expr) == 0, "a matrix of a user value type multiplies a vex::vector<rhs_of<V>::type> only");
+            return direct_product<single_device_matrix, Expr>(A, x);
+        }
+    private:
+        std::vector<backend::command_queue> q;
+        size_t n, m, nnz;
+        std::shared_ptr<const std::array<std::string, 5>> src;     // device names of V and X, decl, product, append
+        std::shared_ptr<vexb_usrmat> A;
 };
 
 template <typename Val, typename Col = int, typename Ptr = Col> using csr   = single_device_matrix<VEXB_FMT_CSR,  Val, Col, Ptr>;

@@ -25,6 +25,23 @@ template <class T> using vec2 = vecn<T, 2>;
 /// Smallest CL vector width that holds n components (vexcl/types.hpp cl_fit_vec_size): 1, 2, 4, 8 or 16.
 template <unsigned n> struct cl_fit_vec_size { static const unsigned value = n <= 1 ? 1 : n <= 2 ? 2 : n <= 4 ? 4 : n <= 8 ? 8 : 16; };
 
+/// Declares a type usable as a vector element and a sparse matrix value (vexcl/types.hpp).  Arithmetic types are; a
+/// user type V that is specialised true here (and has a vex::sparse::spmv_ops_impl) is a user value type, below.
+template <class T> struct is_cl_native : std::is_arithmetic<T> {};
+
+namespace detail {
+template <class T> struct is_std_array : std::false_type {};
+template <class T, size_t N> struct is_std_array<std::array<T, N>> : std::true_type {};
+template <class T> struct is_std_complex : std::false_type {};
+template <class T> struct is_std_complex<std::complex<T>> : std::true_type {};
+}
+
+/// A user value type: declared by is_cl_native, neither arithmetic nor a block (std::array) nor std::complex, which have
+/// kernels of their own.  Sparse matrices of it multiply through its spmv_ops_impl (sparse/spmv_ops.hpp, sparse/matrix.hpp).
+template <class T> struct is_user_value
+    : std::integral_constant<bool, is_cl_native<T>::value && !std::is_arithmetic<T>::value && !detail::is_std_array<T>::value &&
+                                   !detail::is_std_complex<T>::value> {};
+
 template <class T, class Enable = void> struct dtype_of;   // no definition: unsupported element type
 #define VEXB_DTYPE(T, code, nm) \
     template <> struct dtype_of<T> { static const int value = code; static const char *name() { return nm; } };
@@ -66,9 +83,28 @@ template <class T> struct dtype_of<std::complex<T>> {
     static const char *name() { return "complex"; }
 };
 
-template <class T> inline std::string type_name() { return dtype_of<typename std::decay<T>::type>::name(); }
+// User value types are the element of vex::vector<X> and the value of sparse matrices of them (sparse/matrix.hpp): as with
+// blocks, only their products write them.
+template <class T> struct dtype_of<T, typename std::enable_if<is_user_value<T>::value>::type> {
+    static_assert(sizeof(T) == 0, "vex::vector<T> of a user value type (is_cl_native<T>) holds values no expression kernel "
+                                  "knows: the only expressions on them are Y = A * X and Y += A * X with a vex::sparse::{csr, "
+                                  "ell, matrix} of a user value type");
+    static const int value = -1;
+    static const char *name() { return "user"; }
+};
 
-template <class T> struct is_cl_native : std::is_arithmetic<T> {};
+/// Device name of a type (vexcl/types.hpp type_name_impl).  The built-in scalars keep the names of dtype_of; users
+/// specialise it for their value types, whose names go into the generated sparse product kernel (spmv_ops.hpp).
+template <class T, class Enable = void> struct type_name_impl {
+    static std::string get() {
+        static_assert(!is_user_value<T>::value, "a user value type needs a specialisation of vex::type_name_impl<T> whose "
+                                                "get() returns its device type name");
+        return dtype_of<T>::name();
+    }
+};
+
+template <class T> inline std::string type_name() { return type_name_impl<typename std::decay<T>::type>::get(); }
+
 template <class T> struct cl_scalar_of { typedef T type; };
 template <class T> struct cl_vector_length { static const unsigned value = 1; };
 

@@ -204,7 +204,11 @@ class vector : public vector_expr_tag {
         // block sparse products (sparse/matrix.hpp): one launch straight into y
         template <class M> const vector& operator=(const direct_product<M, vector> &p)  { p.A.mul(p.x, *this, 1, false); return *this; }
         template <class M> const vector& operator+=(const direct_product<M, vector> &p) { p.A.mul(p.x, *this, 1, true);  return *this; }
-        template <class M> const vector& operator-=(const direct_product<M, vector> &p) { p.A.mul(p.x, *this, -1, true); return *this; }
+        template <class M> const vector& operator-=(const direct_product<M, vector> &p) {
+            static_assert(detail::direct_scales<M>::value, "a product of a matrix of user value types is not negated: its "
+                          "spmv_ops_impl has no hook for it, so only Y = A * X and Y += A * X are defined");
+            p.A.mul(p.x, *this, -1, true); return *this;
+        }
         const vector& operator=(const detail::additive_terms<T> &a)  { apply_terms(a, T(1), false); return *this; }
         const vector& operator+=(const detail::additive_terms<T> &a) { apply_terms(a, T(1), true);  return *this; }
         const vector& operator-=(const detail::additive_terms<T> &a) { apply_terms(a, T(-1), true); return *this; }

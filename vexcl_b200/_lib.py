@@ -68,6 +68,16 @@ class ZspmatInfo(C.Structure):
                 ("n_slices", C.c_size_t), ("n_slots", C.c_size_t), ("device_bytes", C.c_size_t)]
 
 
+class UsrmatInfo(C.Structure):
+    _fields_ = [("nrows", C.c_size_t), ("ncols", C.c_size_t), ("nnz", C.c_size_t), ("val_bytes", C.c_int32),
+                ("n_slices", C.c_size_t), ("n_slots", C.c_size_t), ("device_bytes", C.c_size_t)]
+
+
+class UsrOps(C.Structure):
+    _fields_ = [("val_type", C.c_char_p), ("rhs_type", C.c_char_p), ("rhs_bytes", C.c_size_t),
+                ("decl", C.c_char_p), ("product", C.c_char_p), ("append", C.c_char_p)]
+
+
 class CcsrInfo(C.Structure):
     _fields_ = [("nrows", C.c_size_t), ("unique_rows", C.c_size_t), ("nnz", C.c_size_t), ("idx_bytes", C.c_int32),
                 ("table_in_smem", C.c_int32), ("device_bytes", C.c_size_t)]
@@ -172,6 +182,11 @@ def lib():
         "vexb_zspmat_destroy": ([vp], i),
         "vexb_zspmat_get_info": ([vp, P(ZspmatInfo)], i),
         "vexb_zspmv": ([i, vp, vp, vp, vp, d, i], i),
+        "vexb_usr_create": ([i, vp, sz, sz, vp, i, vp, i, vp, i, P(vp)], i),
+        "vexb_usrmat_destroy": ([vp], i),
+        "vexb_usrmat_get_info": ([vp, P(UsrmatInfo)], i),
+        "vexb_usr_spmv": ([i, vp, vp, P(UsrOps), vp, vp, i], i),
+        "vexb_jit_source_usr": ([P(UsrOps), i, C.c_char_p, P(sz), i], i),
         "vexb_ccsr_create": ([i, vp, sz, sz, vp, i, vp, i, vp, i, vp, i, P(vp)], i),
         "vexb_ccsr_destroy": ([vp], i),
         "vexb_ccsr_get_info": ([vp, P(CcsrInfo)], i),

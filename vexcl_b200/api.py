@@ -1161,6 +1161,60 @@ class ComplexMatrix:
         return y
 
 
+class UserValueMatrix:
+    """vex::sparse::matrix<V> of a user value type V with its spmv_ops_impl<V, X> (the reference's sparse/spmv_ops.hpp).
+    val has shape (nnz, k): row j is the bytes of value j (k * itemsize bytes, a multiple of 4 up to 64).  val_type and
+    rhs_type name the device types of V and X (e.g. "double4", "double2"), rhs_bytes is sizeof(X).  decl, product and
+    append are the snippets of decl_accum_var(src, "sum"), append_product(src, "sum", "v", "xv") and append(src, "t",
+    "sum").  x and y are plain vectors of scalars holding the bytes of m and n X.  Single device."""
+
+    def __init__(self, ctx: Context, n: int, m: int, ptr, col, val, val_type: str, rhs_type: str, rhs_bytes: int,
+                 decl: str, product: str, append: str):
+        if ctx.nparts != 1:
+            raise ValueError("sparse matrices of user value types are only supported for single-device contexts")
+        self.ctx, self.n, self.m = ctx, int(n), int(m)
+        ptr, col, val = np.ascontiguousarray(ptr), np.ascontiguousarray(col), np.ascontiguousarray(val)
+        if ptr.dtype.itemsize not in (4, 8) or col.dtype.itemsize not in (4, 8):
+            raise TypeError("ptr/col must be 32- or 64-bit integers")
+        if val.ndim != 2:
+            raise ValueError("val must have shape (nnz, k): one row of value bytes per stored entry")
+        self.nnz = int(val.shape[0])
+        self.val_bytes = int(val.shape[1] * val.dtype.itemsize)
+        self.rhs_bytes = int(rhs_bytes)
+        self._strs = [s.encode() for s in (val_type, rhs_type, decl, product, append)]      # kept alive for ops
+        vt, rt, d, p, a = self._strs
+        self.ops = L.UsrOps(vt, rt, self.rhs_bytes, d, p, a)
+        self.h = C.c_void_p()
+        k = ctx.local[0]
+        L.check(L.lib().vexb_usr_create(ctx.devs[k], ctx.streams[k], self.n, self.m, _ip(ptr), ptr.dtype.itemsize,
+                                        _ip(col), col.dtype.itemsize, _ip(val), self.val_bytes, C.byref(self.h)))
+
+    def __del__(self):
+        try:
+            L.lib().vexb_usrmat_destroy(self.h)
+        except Exception:
+            pass
+
+    def rows(self): return self.n
+    def cols(self): return self.m
+    def nonzeros(self): return self.nnz
+
+    def info(self) -> L.UsrmatInfo:
+        info = L.UsrmatInfo()
+        L.check(L.lib().vexb_usrmat_get_info(self.h, C.byref(info)))
+        return info
+
+    def apply(self, x: vector, y: vector, append: bool = False):
+        """y = A*x  or  y += A*x, one launch of the generated kernel (compiled at the first call on a device)."""
+        xb, yb = x.n * x.np_dtype.itemsize, y.n * y.np_dtype.itemsize
+        if xb != self.m * self.rhs_bytes or yb != self.n * self.rhs_bytes:
+            raise ValueError("UserValueMatrix::apply: vector sizes do not match the matrix")
+        k = self.ctx.local[0]
+        L.check(L.lib().vexb_usr_spmv(self.ctx.devs[k], self.ctx.streams[k], self.h, C.byref(self.ops), x.bufs[k], y.bufs[k],
+                                      int(append)))
+        return y
+
+
 class stencil:
     """vex::stencil<T> (stencil.hpp:168-330): `y = x * s`, `y += x * s`, `y = 42 * (x * s)`, ...
     y[i] = sum_k s[k] * x[clamp(i + k - center)]; with several slices the neighbours' edge elements are copied

@@ -10,8 +10,16 @@
 // B*B values: 8B^2 + 4 bytes per stored block in double against 12B^2 for the same block expanded into scalar CSR.
 // Complex strips are the same layout over rows with 2 components per slot, c = 0 (re) and c = 1 (im): 2 sizeof(T) + 4
 // bytes per stored entry, and one 2 sizeof(T)-byte gather of x (re, im) per slot.
+// User strips (vex::sparse::{csr, ell, matrix}<V> for a user type V with a vex::sparse::spmv_ops_impl<V, X>) are the same
+// layout over rows with ONE opaque component of val_bytes per slot: lane l of slot k in slice s holds the value at index
+// slice_ptr[s] + 32k + l, so a warp's value loads are 32 consecutive V.  Their kernel is generated from the user's source
+// snippets and compiled by NVRTC at first use (usr_source below).
 #include "hostlogic.hpp"
+#include "jit.hpp"
 #include "spmv_dev.cuh"
+#include <map>
+#include <mutex>
+#include <sstream>
 #include <vector>
 
 namespace vexb {
@@ -30,6 +38,11 @@ struct vexb_bspmat : vexb::sell_strip {
 struct vexb_zspmat : vexb::sell_strip {
     int dev = 0, val_dtype = VEXB_F64;         // VEXB_F64: std::complex<double>, VEXB_F32: std::complex<float>
     size_t nrows = 0, ncols = 0, nnz = 0;      // rows, columns, stored complex entries
+};
+
+struct vexb_usrmat : vexb::sell_strip {
+    int dev = 0, val_bytes = 0;                // sizeof(V)
+    size_t nrows = 0, ncols = 0, nnz = 0;      // rows, columns, stored values
 };
 
 namespace vexb {
@@ -196,11 +209,10 @@ struct sell_host {
     size_t nnz = 0, slots = 0;
 };
 
-// The argument checks of vexb_bsr_create and vexb_zsr_create; none touches a device.  `unit` is "block " when rows,
+// The argument checks of vexb_bsr_create, vexb_zsr_create and vexb_usr_create but the value type's; none touches a device.  `unit` is "block " when rows,
 // columns and entries count blocks, "" otherwise.
 static int sell_check(size_t nrows, size_t ncols, const void *ptr, int ptr_bytes, const void *col, int col_bytes,
-                      const void *val, int val_dtype, const char *unit, sell_host &h) {
-    VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
+                      const void *val, const char *unit, sell_host &h) {
     VEXB_CHECK(ptr_bytes == 4 || ptr_bytes == 8, "ptr_bytes must be 4 or 8");
     VEXB_CHECK(col_bytes == 4 || col_bytes == 8, "col_bytes must be 4 or 8");
     VEXB_CHECK(nrows == 0 || ptr, "ptr is NULL");
@@ -227,13 +239,13 @@ static int sell_check(size_t nrows, size_t ncols, const void *ptr, int ptr_bytes
     return VEXB_OK;
 }
 
-// Host packing of the planar slots (see the top of this file), `comps` values per stored entry; padding slots keep
-// column -1 and zero values.
-template <class T>
-static int sell_upload(sell_strip *S, const sell_host &h, const T *val, size_t comps) {
+// Host packing of the planar slots (see the top of this file), `comps` components of `comp_bytes` bytes per stored entry;
+// padding slots keep column -1 and zero bytes.
+static int sell_upload(sell_strip *S, const sell_host &h, const void *val, size_t comp_bytes, size_t comps) {
     S->n_slices = h.sptr.size() - 1; S->n_slots = h.slots;
     std::vector<int> scol(S->n_slots, -1);
-    std::vector<T> sval(S->n_slots * comps, T(0));
+    std::vector<unsigned char> sval(S->n_slots * comps * comp_bytes, 0);
+    const unsigned char *src = static_cast<const unsigned char *>(val);
     for (size_t sl = 0; sl < S->n_slices; ++sl)
         for (int l = 0; l < 32; ++l) {
             const int r = h.perm[sl * 32 + l];
@@ -241,19 +253,19 @@ static int sell_upload(sell_strip *S, const sell_host &h, const T *val, size_t c
             for (int j = h.rp[r], k = 0; j < h.rp[r + 1]; ++j, ++k) {
                 const size_t slot = (size_t)h.sptr[sl] + (size_t)k * 32;
                 scol[slot + l] = h.col[j];
-                for (size_t c = 0; c < comps; ++c) sval[slot * comps + 32 * c + l] = val[(size_t)j * comps + c];
+                for (size_t c = 0; c < comps; ++c)
+                    memcpy(&sval[(slot * comps + 32 * c + l) * comp_bytes], src + ((size_t)j * comps + c) * comp_bytes, comp_bytes);
             }
         }
     VEXB_TRY(upload_array(h.sptr, (void **)&S->slice_ptr, &S->device_bytes));
     VEXB_TRY(upload_array(h.perm, (void **)&S->perm, &S->device_bytes));
     VEXB_TRY(upload_array(scol, (void **)&S->col, &S->device_bytes));
     VEXB_TRY(upload_array(sval, &S->val, &S->device_bytes));
+    // cudaMemcpy from pageable memory may return before its DMA has landed, and the products run on non-blocking streams,
+    // which do not wait for the legacy stream: without this, a product launched right after create() can read a tail of
+    // values that is not there yet
+    VEXB_CUDA(cudaStreamSynchronize(0));
     return VEXB_OK;
-}
-
-static int sell_upload(sell_strip *S, const sell_host &h, const void *val, int val_dtype, size_t comps) {
-    return val_dtype == VEXB_F64 ? sell_upload<double>(S, h, (const double *)val, comps)
-                                 : sell_upload<float>(S, h, (const float *)val, comps);
 }
 
 static void sell_free(sell_strip *S) {
@@ -271,15 +283,16 @@ extern "C" int vexb_bsr_create(int dev, void *stream, size_t nrows, size_t ncols
     VEXB_CHECK(out, "out is NULL");
     *out = nullptr;
     VEXB_CHECK(block >= 2 && block <= 4, "block size %d is not 2, 3 or 4", block);
+    VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
     sell_host h;
-    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, val_dtype, "block ", h));
+    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, "block ", h));
 
     DeviceGuard g(dev);
     if (!g.ok) VEXB_FAIL(VEXB_ERR_CUDA, "cannot select device %d", dev);
     vexb_bspmat *A = new vexb_bspmat;
     A->dev = dev; A->block = block; A->val_dtype = val_dtype;
     A->nrows = nrows; A->ncols = ncols; A->nnzb = h.nnz;
-    const int st = sell_upload(A, h, val, val_dtype, (size_t)block * block);
+    const int st = sell_upload(A, h, val, dtype_size(val_dtype), (size_t)block * block);
     if (st != VEXB_OK) { vexb_bspmat_destroy(A); return st; }
     *out = A;
     return VEXB_OK;
@@ -319,15 +332,16 @@ extern "C" int vexb_zsr_create(int dev, void *stream, size_t nrows, size_t ncols
     // every argument is checked before a device is touched (tests/test_zsr_oracle.py runs these checks without one)
     VEXB_CHECK(out, "out is NULL");
     *out = nullptr;
+    VEXB_CHECK(val_dtype == VEXB_F64 || val_dtype == VEXB_F32, "values must be f64 or f32");
     sell_host h;
-    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, val_dtype, "", h));
+    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, "", h));
 
     DeviceGuard g(dev);
     if (!g.ok) VEXB_FAIL(VEXB_ERR_CUDA, "cannot select device %d", dev);
     vexb_zspmat *A = new vexb_zspmat;
     A->dev = dev; A->val_dtype = val_dtype;
     A->nrows = nrows; A->ncols = ncols; A->nnz = h.nnz;
-    const int st = sell_upload(A, h, val, val_dtype, 2);          // (re, im) of each entry: the bytes of std::complex<T>
+    const int st = sell_upload(A, h, val, dtype_size(val_dtype), 2);   // (re, im) of each entry: the bytes of std::complex<T>
     if (st != VEXB_OK) { vexb_zspmat_destroy(A); return st; }
     *out = A;
     return VEXB_OK;
@@ -361,4 +375,199 @@ extern "C" int vexb_zspmv(int dev, void *stream, const vexb_zspmat *A, const voi
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     if (A->val_dtype == VEXB_F64) return zspmv_launch<double>(A, (cudaStream_t)stream, (const double *)x, (double *)y, alpha, append);
     return zspmv_launch<float>(A, (cudaStream_t)stream, (const float *)x, (float *)y, (float)alpha, append);
+}
+
+// ---- user value types -------------------------------------------------------------------------------------------------
+namespace vexb {
+
+// Slots in flight per loop turn of the generated kernel: U * (1 value + 1 column) streaming loads and U gathers of x per
+// lane.  No spills for the 2 x 2 block (double4 / double2) or the complex (double2) type in either precision
+// (-Xptxas -v on the generated source, DESIGN.md section 3 lists the register counts).
+constexpr int kUsellUnroll = 4;
+
+// Device type names are spelled by the user's type_name_impl: identifiers, possibly qualified or with spaces
+// ("unsigned int").  Anything else (a brace, a semicolon) would put code outside the snippets.
+static bool type_name_ok(const char *t) {
+    if (!t || !*t) return false;
+    for (const char *c = t; *c; ++c)
+        if (!isalnum((unsigned char)*c) && *c != '_' && *c != ':' && *c != ' ') return false;
+    return true;
+}
+
+static int usr_check_ops(const vexb_usr_ops *o) {
+    VEXB_CHECK(o, "ops is NULL");
+    VEXB_CHECK(type_name_ok(o->val_type), "val_type is not a type name");
+    VEXB_CHECK(type_name_ok(o->rhs_type), "rhs_type is not a type name");
+    VEXB_CHECK(o->rhs_bytes >= 1 && o->rhs_bytes <= 64, "rhs_bytes %zu is not in 1..64", o->rhs_bytes);
+    VEXB_CHECK(o->decl && o->product && o->append, "a snippet of ops is NULL");
+    return VEXB_OK;
+}
+
+// Alignment of a device vector type of `bytes` bytes (double2: 16, double3: 8, float2: 8, float3: 4, double4: 16).
+static size_t natural_align(size_t bytes) {
+    size_t a = 1;
+    while (a < 16 && bytes % (2 * a) == 0) a *= 2;
+    return a;
+}
+
+// The product kernel of a user strip (one warp per slice, one lane per row, as zsell_kernel), with the spmv_ops_impl
+// snippets of the value type V and the vector type X, which use the names `sum` (accumulator), `v` (matrix value), `xv`
+// (x at its column) and `t` (the old y_r in y += A x).  Per row, in storage order: decl; then for every stored value
+// append_product(sum, v, xv); then y_r = sum, or t = y_r, append(t, sum), y_r = t.  Padding slots are skipped.
+static std::string usr_source(const vexb_usr_ops &o, size_t val_bytes) {
+    const int U = kUsellUnroll;
+    std::ostringstream s;
+    s << "// generated by libvexb200 (csrc/bspmv.cu): sliced-ELL product of a user value type\n"
+         "typedef " << o.val_type << " vexb_val_t;\n"
+         "typedef " << o.rhs_type << " vexb_rhs_t;\n"
+         "static_assert(sizeof(vexb_val_t) == " << val_bytes << " && sizeof(vexb_rhs_t) == " << o.rhs_bytes << ",\n"
+         "              \"the device types " << o.val_type << " and " << o.rhs_type << " must have the sizes of the host value "
+         "(" << val_bytes << " bytes) and vector (" << o.rhs_bytes << " bytes) types\");\n"
+         "extern \"C\" __global__ void __launch_bounds__(256) vexb_usr_kernel(unsigned long long n_slices_,\n"
+         "    const int *__restrict__ slice_ptr_, const int *__restrict__ perm_, const int *__restrict__ col_,\n"
+         "    const vexb_val_t *__restrict__ val_, const vexb_rhs_t *__restrict__ x_, vexb_rhs_t *y_, int append_) {\n"
+         "  const unsigned long long s_ = (unsigned long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);\n"
+         "  if (s_ >= n_slices_) return;\n"
+         "  const int lane_ = threadIdx.x & 31;\n"
+         "  const int base_ = __ldg(slice_ptr_ + s_), w_ = (__ldg(slice_ptr_ + s_ + 1) - base_) >> 5;\n"
+         "  const int *cp_ = col_ + base_ + lane_;\n"
+         "  const vexb_val_t *vp_ = val_ + (unsigned long long)base_ + lane_;\n" << o.decl << "\n"
+         "  int k_ = 0;\n"
+         "  for (; k_ + " << U << " <= w_; k_ += " << U << ") {\n"
+         "    int c_[" << U << "]; vexb_val_t a_[" << U << "]; vexb_rhs_t b_[" << U << "];\n"
+         "#pragma unroll\n"
+         "    for (int u_ = 0; u_ < " << U << "; ++u_) { c_[u_] = __ldcs(cp_ + (k_ + u_) * 32); a_[u_] = vp_[(unsigned long long)(k_ + u_) * 32]; }\n"
+         "#pragma unroll\n"
+         "    for (int u_ = 0; u_ < " << U << "; ++u_) if (c_[u_] != -1) b_[u_] = x_[c_[u_]];\n"
+         "#pragma unroll\n"
+         "    for (int u_ = 0; u_ < " << U << "; ++u_) if (c_[u_] != -1) {\n"
+         "      const vexb_val_t v = a_[u_]; const vexb_rhs_t xv = b_[u_];\n" << o.product << "\n"
+         "    }\n"
+         "  }\n"
+         "  for (; k_ < w_; ++k_) {\n"
+         "    const int c_ = __ldcs(cp_ + k_ * 32);\n"
+         "    const vexb_val_t a_ = vp_[(unsigned long long)k_ * 32];\n"
+         "    if (c_ != -1) {\n"
+         "      const vexb_val_t v = a_; const vexb_rhs_t xv = x_[c_];\n" << o.product << "\n"
+         "    }\n"
+         "  }\n"
+         "  const int r_ = __ldcs(perm_ + s_ * 32 + lane_);\n"     // read last: a register less through the loops
+         "  if (r_ >= 0) {\n"
+         "    if (append_) {\n"
+         "      vexb_rhs_t t = y_[r_];\n" << o.append << "\n"
+         "      y_[r_] = t;\n"
+         "    } else {\n"
+         "      y_[r_] = sum;\n"
+         "    }\n"
+         "  }\n"
+         "}\n";
+    return s.str();
+}
+
+// Compiled kernels by (snippets, val_bytes, device): the front ends pass the same ops on every call, and this key is much
+// shorter than the source jit_build would otherwise compare.
+static std::mutex g_usr_mx;
+static std::map<std::pair<std::string, int>, void *> g_usr_fns;
+
+static int usr_kernel(int dev, const vexb_usr_ops &o, size_t val_bytes, void **fn) {
+    std::string key;
+    for (const char *part : {o.val_type, o.rhs_type, o.decl, o.product, o.append}) {
+        key += std::to_string(strlen(part)); key += ':'; key += part;
+    }
+    key += std::to_string(o.rhs_bytes) + ":" + std::to_string(val_bytes);
+    const auto k = std::make_pair(key, dev);
+    {
+        std::lock_guard<std::mutex> lock(g_usr_mx);
+        auto it = g_usr_fns.find(k);
+        if (it != g_usr_fns.end()) { *fn = it->second; return VEXB_OK; }
+    }
+    VEXB_TRY(jit_build(dev, usr_source(o, val_bytes), "vexb_usr_kernel", fn));
+    std::lock_guard<std::mutex> lock(g_usr_mx);
+    g_usr_fns[k] = *fn;
+    return VEXB_OK;
+}
+
+} // namespace vexb
+
+extern "C" int vexb_usr_create(int dev, void *stream, size_t nrows, size_t ncols, const void *ptr, int ptr_bytes,
+                               const void *col, int col_bytes, const void *val, int val_bytes, vexb_usrmat **out) {
+    (void)stream;
+    // every argument is checked before a device is touched (tests/test_usr_jit_cpu.py runs these checks without one)
+    VEXB_CHECK(out, "out is NULL");
+    *out = nullptr;
+    VEXB_CHECK(val_bytes >= 1 && val_bytes <= 64 && val_bytes % 4 == 0, "val_bytes %d is not a multiple of 4 in 4..64", val_bytes);
+    sell_host h;
+    VEXB_TRY(sell_check(nrows, ncols, ptr, ptr_bytes, col, col_bytes, val, "", h));
+
+    DeviceGuard g(dev);
+    if (!g.ok) VEXB_FAIL(VEXB_ERR_CUDA, "cannot select device %d", dev);
+    vexb_usrmat *A = new vexb_usrmat;
+    A->dev = dev; A->val_bytes = val_bytes;
+    A->nrows = nrows; A->ncols = ncols; A->nnz = h.nnz;
+    const int st = sell_upload(A, h, val, (size_t)val_bytes, 1);
+    if (st != VEXB_OK) { vexb_usrmat_destroy(A); return st; }
+    *out = A;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_usrmat_destroy(vexb_usrmat *A) {
+    if (!A) return VEXB_OK;
+    VEXB_RELEASE_GUARD();
+    DeviceGuard g(A->dev);
+    sell_free(A);
+    delete A;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_usrmat_get_info(const vexb_usrmat *A, vexb_usrmat_info *info) {
+    VEXB_CHECK(A && info, "NULL argument");
+    memset(info, 0, sizeof(*info));
+    info->nrows = A->nrows; info->ncols = A->ncols; info->nnz = A->nnz;
+    info->val_bytes = A->val_bytes;
+    info->n_slices = A->n_slices; info->n_slots = A->n_slots; info->device_bytes = A->device_bytes;
+    return VEXB_OK;
+}
+
+extern "C" int vexb_usr_spmv(int dev, void *stream, const vexb_usrmat *A, const vexb_usr_ops *ops, const void *x, void *y, int append) {
+    VEXB_CHECK(A, "matrix is NULL");
+    VEXB_TRY(usr_check_ops(ops));
+    VEXB_CHECK(dev == A->dev, "matrix lives on device %d, not %d", A->dev, dev);
+    VEXB_CHECK(A->nrows == 0 || y, "y is NULL");
+    VEXB_CHECK(A->nnz == 0 || x, "x is NULL");
+    const size_t al = natural_align(ops->rhs_bytes);
+    VEXB_CHECK((uintptr_t)x % al == 0 && (uintptr_t)y % al == 0, "x and y must be aligned to %zu bytes", al);
+    DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
+    if (A->nrows == 0) return VEXB_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (A->nnz == 0) {
+        // as vexb_spmv on an empty strip: y = A*x zeroes y, y += A*x leaves it alone
+        if (!append) VEXB_CUDA(cudaMemsetAsync(y, 0, A->nrows * ops->rhs_bytes, st));
+        return VEXB_OK;
+    }
+    void *fn = nullptr;
+    VEXB_TRY(usr_kernel(dev, *ops, (size_t)A->val_bytes, &fn));
+    unsigned long long ns = A->n_slices;
+    const void *sp = A->slice_ptr, *pm = A->perm, *cl = A->col, *vl = A->val;
+    int ap = append ? 1 : 0;
+    void *args[] = {&ns, &sp, &pm, &cl, &vl, &x, &y, &ap};
+    return jit_launch(fn, (unsigned)((A->n_slices + 7) / 8), 256, 0, st, args);
+}
+
+extern "C" int vexb_jit_source_usr(const vexb_usr_ops *ops, int val_bytes, char *buf, size_t *len, int compile) {
+    VEXB_CHECK(len, "len is NULL");
+    VEXB_TRY(usr_check_ops(ops));
+    VEXB_CHECK(val_bytes >= 1 && val_bytes <= 64 && val_bytes % 4 == 0, "val_bytes %d is not a multiple of 4 in 4..64", val_bytes);
+    std::string src = usr_source(*ops, (size_t)val_bytes);
+    if (compile) {
+        size_t cubin = 0; std::string log;
+        VEXB_TRY(jit_compile_only(src, &cubin, &log));
+        src += "// NVRTC: ok, cubin " + std::to_string(cubin) + " bytes\n";
+        if (!log.empty()) src += "/* log:\n" + log + "*/\n";
+    }
+    if (buf) {
+        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
+        memcpy(buf, src.c_str(), src.size() + 1);
+    }
+    *len = src.size() + 1;
+    return VEXB_OK;
 }
