@@ -106,7 +106,8 @@ typedef enum {
     VEXB_TERM_INDEX = 2,  /* element_index: index_offset + i + v.i64 (element_index.hpp:40-111), type u64 */
     VEXB_TERM_DSCALAR = 3,/* v.ptr: ONE device-resident value of `dtype`, broadcast to every element.  Lets the
                              result of vexb_reduce feed the next expression without a host round trip. */
-    VEXB_TERM_SPMV = 4    /* v.ptr: a vexb_spmat (host handle; CSR or hybrid ELL, plain strip); pad[0]: slot of the
+    VEXB_TERM_SPMV = 4    /* v.ptr: a vexb_spmat (host handle; CSR or hybrid ELL, plain strip -- or, in vexb_eval only,
+                             sliced ELL: see vexb_dspmat_sweep_strip); pad[0]: slot of the
                              VEXB_TERM_VEC holding x.  Element i evaluates to row i of A*x (products added in storage
                              order, as vexb_spmv does): the sparse product as a *terminal* of the consumer's kernel --
                              `y = x + A*x` is one launch, y is written once and A*x never goes to memory
@@ -643,6 +644,14 @@ int vexb_dspmat_download_split(const vexb_dspmat *A, int64_t *loc_ptr, int64_t *
 /* The part's strip for use as a VEXB_TERM_SPMV terminal: set when the part has no ghost columns and its rows are
  * stored plainly in CSR or hybrid ELL (then row i of the strip is element i of the part's slice); NULL otherwise. */
 int vexb_dspmat_inline_strip(const vexb_dspmat *A, const vexb_spmat **strip);
+/* The part's strip for use as a VEXB_TERM_SPMV terminal of an ASSIGNMENT (vexb_eval): set when the part has no ghost
+ * columns and its rows are stored plainly in sliced ELL with values of the vector type, and the tunables
+ * "spmv.sell_inline" (default 1) and "spmv.no_inline" (default 0) allow it; NULL otherwise.  The generated kernel then
+ * sweeps in the strip's storage order -- one thread per stored lane, every operand and the target at that lane's row --
+ * so the column and value loads stay coalesced as in the plain product.  One distinct sliced-ELL strip per expression,
+ * any number of times (`A*x + A*z`); a second one is VEXB_ERR_UNSUPPORTED.  vexb_eval_multi and the reductions
+ * (vexb_reduce_all, vexb_reduce_multi) do not take such strips. */
+int vexb_dspmat_sweep_strip(const vexb_dspmat *A, const vexb_spmat **strip);
 void *vexb_dspmat_send_buffer(const vexb_dspmat *A);  /* device, n_send values  */
 void *vexb_dspmat_ghost_buffer(const vexb_dspmat *A); /* device, n_ghost values */
 /* Steps of SpMat::apply, all asynchronous on `stream`: */
@@ -672,8 +681,8 @@ int vexb_dspmat_apply(int nlocal, vexb_comm *const *comms, vexb_dspmat *const *p
                       const void *const *x, void *const *y, double alpha, int append);
 
 /* Several right-hand sides in one pass over the matrix: vex::SpMat * vex::multivector<T,N> (multivector.hpp;
- * the reference multiplies component by component, operations.hpp:876-880).  Hybrid-ELL strips take groups of up to 4
- * vectors per launch (columns and values loaded once, same per-component bits as vexb_spmv); anything else falls back to
+ * the reference multiplies component by component, operations.hpp:876-880).  Hybrid-ELL and sliced-ELL strips take groups
+ * of up to 4 vectors per launch (columns and values loaded once, same per-component bits as vexb_spmv); anything else falls back to
  * one product per vector.  vexb_dspmat_apply_multi: x[k * nrhs + r] / y[k * nrhs + r] = slice of component r on part k;
  * parts with a halo multiply component by component. */
 int vexb_spmv_multi(int dev, void *stream, const vexb_spmat *A, int nrhs, const void *const *x, void *const *y,

@@ -98,6 +98,17 @@ struct expr_props {
     size_t size = 0;
     bool sized = false;
     int comp = -1;                  ///< component being prepared (multi-expressions), else -1
+    /// Assignments only (assign_expression): the generated kernel may sweep in the storage order of ONE sliced-ELL strip
+    /// (vexb_dspmat_sweep_strip).  The first product that asks claims it; products of other such matrices take a temporary.
+    bool sweeps = false;
+    const vexb_spmat *swept = nullptr;
+    template <class M> bool claim_sweep(const M &A) {
+        if (!sweeps || A.queue_list().empty()) return false;
+        for (unsigned d = 0; d < A.queue_list().size(); ++d) if (!A.sweep_strip(d)) return false;
+        if (swept && swept != A.sweep_strip(0)) return false;
+        swept = A.sweep_strip(0);
+        return true;
+    }
 
     void see(const std::vector<backend::command_queue> &q, const std::vector<size_t> &p, size_t n) {
         if (!queue) { queue = &q; part = p; }
@@ -342,6 +353,7 @@ struct additive_terms {
     struct term {
         std::function<void(vex::vector<T>&, T, bool)> apply;       ///< y (=|+=) sign * scale * A * x
         std::function<bool(unsigned)> can_inline;                    ///< on device d
+        std::function<const vexb_spmat*(unsigned)> sweep_strip;      ///< device d's sliced-ELL strip for a storage-order sweep, or NULL
         std::function<void(ir_builder&, T)> lower;                   ///< pushes sign * scale * (A*x)_i
         void operator()(vex::vector<T> &y, T sign, bool append) const { apply(y, sign, append); }
     };
@@ -354,6 +366,7 @@ struct additive_terms {
             term u;
             u.apply = [t, s](vex::vector<T> &y, T sign, bool append) { t.apply(y, sign * s, append); };
             u.can_inline = t.can_inline;
+            u.sweep_strip = t.sweep_strip;
             u.lower = [t, s](ir_builder &b, T sign) { t.lower(b, sign * s); };
             r.terms.push_back(u);
         }
@@ -369,10 +382,12 @@ struct additive_terms {
             term t;
             t.apply = [a](vex::vector<T> &y, T sign, bool append) { a.apply(y, sign, append); };
             t.can_inline = [a](unsigned d) { return a.A.inline_strip(d) != nullptr; };
+            t.sweep_strip = [a](unsigned d) { return a.A.sweep_strip(d); };
             t.lower = [a](ir_builder &b, T sign) {
                 const int dt = dtype_of<T>::value;
                 b.push_scalar(static_cast<T>(sign * a.scale));
-                b.push_spmv(a.A.inline_strip(b.part), a.x(b.part).raw(), dt);
+                const vexb_spmat *s = a.A.inline_strip(b.part);
+                b.push_spmv(s ? s : a.A.sweep_strip(b.part), a.x(b.part).raw(), dt);
                 b.emit(VEXB_OP_MUL, dt);
             };
             return t;
@@ -382,6 +397,7 @@ struct additive_terms {
             term t;
             t.apply = [a](vex::vector<T> &y, T sign, bool append) { a.apply(y, sign, append); };
             t.can_inline = [](unsigned) { return false; };
+            t.sweep_strip = [](unsigned) { return static_cast<const vexb_spmat*>(nullptr); };
             t.lower = [](ir_builder&, T) {};
             return t;
         }
@@ -395,7 +411,11 @@ struct fused_mixed : vector_expr_tag {
     typedef T value_type;
     const E &expr; const additive_terms<T> &terms; T sign;
     fused_mixed(const E &e, const additive_terms<T> &t, T sign) : expr(e), terms(t), sign(sign) {}
-    void props(expr_props &p) const { expr.props(p); }
+    void props(expr_props &p) const {
+        // the terms' sliced-ELL strip (vector::inlinable admits one) is claimed before the vector part asks
+        for (auto &t : terms.terms) if (!t.can_inline(0) && !p.swept) p.swept = t.sweep_strip(0);
+        expr.props(p);
+    }
     int lower(ir_builder &b) const {
         const int dt = dtype_of<T>::value;
         const int et = expr.lower(b);
@@ -488,6 +508,7 @@ template <class OP, class T, class Expr>
 void assign_expression(vex::vector<T> &lhs, const Expr &expr, int comp = -1) {
     expr_props p;
     p.comp = comp;
+    p.sweeps = comp < 0;
     p.see(lhs.queue_list(), lhs.partition(), lhs.size());
     expr.props(p);
     const std::vector<backend::command_queue> &queue = lhs.queue_list();

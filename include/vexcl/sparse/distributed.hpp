@@ -49,6 +49,7 @@ class distributed {
 
         /// Device d's strip when a generated kernel can walk its rows (no halo on that device), else NULL.
         const vexb_spmat* inline_strip(unsigned d) const { return A.inline_strip(d); }
+        const vexb_spmat* sweep_strip(unsigned d) const { return A.sweep_strip(d); }
 
         template <class Expr>
         friend typename std::enable_if<is_vector_expr<Expr>::value, matrix_vector_product<distributed, Expr> >::type

@@ -66,6 +66,18 @@ class single_device_matrix {
             return (i.fmt == VEXB_FMT_CSR || i.fmt == VEXB_FMT_HELL) ? A.get() : nullptr;
         }
 
+        /// The strip when an assignment can take it as a terminal by sweeping in its storage order (sliced ELL with values of
+        /// the vector type, "spmv.sell_inline" on and "spmv.no_inline" off), else NULL.
+        const vexb_spmat* sweep_strip(unsigned = 0) const {
+            vexb_spmat_info i;
+            long on = 1, off = 0;
+            if (!A || vexb_spmat_get_info(A.get(), &i) != VEXB_OK) return nullptr;
+            if (vexb_get_param("spmv.sell_inline", &on) != VEXB_OK) on = 1;       // never set: the default
+            if (vexb_get_param("spmv.no_inline", &off) != VEXB_OK) off = 0;
+            if (i.val_dtype == VEXB_F64 && i.val_bytes == 4) return nullptr;      // VEXB_FMT_VALUES_F32
+            return (i.fmt == VEXB_FMT_SELL && on && !off) ? A.get() : nullptr;
+        }
+
         template <class Expr>
         friend typename std::enable_if<is_vector_expr<Expr>::value, matrix_vector_product<single_device_matrix, Expr> >::type
         operator*(const single_device_matrix &A, const Expr &x) { return matrix_vector_product<single_device_matrix, Expr>(A, x); }

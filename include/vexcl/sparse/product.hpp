@@ -9,7 +9,8 @@
  * specialised to the strip's format (CSR, or hybrid ELL with its width unrolled).  `x` may itself
  * be an expression; it is then evaluated into a temporary first (a gather needs all of x).
  * A reduction such as `sum(f - A*x)` is one generated kernel too: the row loop feeds the fold directly.
- * Row-pattern strips go through a temporary y instead.
+ * In an assignment a sliced-ELL strip is a terminal too: the kernel then sweeps in the strip's storage order (one such
+ * matrix per expression; a reduction of it keeps its temporary).  Row-pattern strips go through a temporary y instead.
  */
 #include <memory>
 #include "../operations.hpp"
@@ -34,6 +35,7 @@ struct matrix_vector_product : vector_expr_tag {
         xv = &materialize(x);
         fused = std::is_floating_point<value_type>::value;
         for (unsigned d = 0; fused && d < A.queue_list().size(); ++d) fused = A.inline_strip(d) != nullptr;
+        if (!fused && std::is_floating_point<value_type>::value) fused = p.claim_sweep(A);     // assignments: a sliced-ELL strip, swept in storage order
         if (fused) { p.see(A.queue_list(), vex::partition(A.rows(), A.queue_list()), A.rows()); return; }   // row loop goes into the consumer's kernel
         if (!y || y->size() != A.rows()) y = std::make_shared<vex::vector<value_type>>(A.queue_list(), A.rows());
         A.mul(*xv, *y);
@@ -41,7 +43,8 @@ struct matrix_vector_product : vector_expr_tag {
     }
     int lower(detail::ir_builder &b) const {
         if (!fused) return y->lower(b);
-        b.push_spmv(A.inline_strip(b.part), (*xv)(b.part).raw(), dtype_of<value_type>::value);
+        const vexb_spmat *s = A.inline_strip(b.part);
+        b.push_spmv(s ? s : A.sweep_strip(b.part), (*xv)(b.part).raw(), dtype_of<value_type>::value);
         return dtype_of<value_type>::value;
     }
     mutable bool fused = false;

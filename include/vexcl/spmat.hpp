@@ -111,6 +111,14 @@ class SpMat {
             if (d < mtx.size() && mtx[d]) vexb_dspmat_inline_strip(mtx[d], &s);
             return s;
         }
+        /// The strip of device d when an assignment can take it as a terminal by sweeping in its storage order (no halo,
+        /// plain sliced ELL), else NULL.
+        const vexb_spmat* sweep_strip(unsigned d) const {
+            const vexb_spmat *s = nullptr;
+            if (d < mtx.size() && mtx[d]) vexb_dspmat_sweep_strip(mtx[d], &s);
+            return s;
+        }
+        const std::vector<backend::command_queue>& queue_list() const { return queue; }
         bool inlinable() const { for (unsigned d = 0; d < mtx.size(); ++d) if (!inline_strip(d)) return false; return !mtx.empty(); }
 
         size_t rows() const { return nrows; }
@@ -152,7 +160,7 @@ struct inline_spmv : vector_expr_tag {
     mutable std::shared_ptr<vex::vector<value_type>> y;
     inline_spmv(const M &A, const V &x) : A(A), x(x) {}
     void props(detail::expr_props &p) const {
-        fused = std::is_floating_point<value_type>::value && A.inlinable() && x.size() == A.cols();
+        fused = std::is_floating_point<value_type>::value && x.size() == A.cols() && (A.inlinable() || p.claim_sweep(A));
         if (fused) { p.see(x.queue_list(), vex::partition(A.rows(), x.queue_list()), A.rows()); return; }   // the row loop goes into the consumer's kernel
         if (!y || y->size() != A.rows()) y = std::make_shared<vex::vector<value_type>>(x.queue_list(), A.rows());
         A.apply(x, *y, 1, false);
@@ -160,7 +168,8 @@ struct inline_spmv : vector_expr_tag {
     }
     int lower(detail::ir_builder &b) const {
         if (!fused) return y->lower(b);
-        b.push_spmv(A.inline_strip(b.part), x(b.part).raw(), dtype_of<value_type>::value);
+        const vexb_spmat *s = A.inline_strip(b.part);
+        b.push_spmv(s ? s : A.sweep_strip(b.part), x(b.part).raw(), dtype_of<value_type>::value);
         return dtype_of<value_type>::value;
     }
     mutable bool fused = false;

@@ -265,7 +265,13 @@ class vector : public vector_expr_tag {
         }
         bool inlinable(const detail::additive_terms<T> &a) const {
             if (a.terms.empty() || a.terms.size() > 6 || !std::is_floating_point<T>::value) return false;
-            for (auto &t : a.terms) for (unsigned d = 0; d < queue.size(); ++d) if (!t.can_inline(d)) return false;
+            // a term is inlined thread per row, or -- one distinct sliced-ELL matrix per assignment -- by a storage-order sweep
+            const vexb_spmat *swept = nullptr;
+            for (auto &t : a.terms) for (unsigned d = 0; d < queue.size(); ++d) {
+                if (t.can_inline(d)) continue;
+                if (!t.sweep_strip(d) || (swept && swept != t.sweep_strip(0))) return false;
+                swept = t.sweep_strip(0);
+            }
             return true;
         }
 };

@@ -214,6 +214,7 @@ def lib():
         "vexb_dspmat_apply_dot": ([i, P(vp), P(vp), P(vp), P(vp), d, i, P(vp), P(vp), P(vp)], i),
         "vexb_peer_fault": ([P(C.c_uint64), i], i),
         "vexb_dspmat_inline_strip": ([vp, P(vp)], i),
+        "vexb_dspmat_sweep_strip": ([vp, P(vp)], i),
         "vexb_spmv_multi": ([i, vp, vp, i, P(vp), P(vp), d, i], i),
         "vexb_dspmat_apply_multi": ([i, P(vp), P(vp), P(vp), i, P(vp), P(vp), d, i], i),
         "vexb_jit_pending": ([P(i)], i),

@@ -342,6 +342,9 @@ class _Lowering:
         self.part, self.part_start = part, part_start
         self.size = None
         self.ctx = None
+        # assignments only: the one matrix whose sliced-ELL strips this expression may take as terminals (the generated
+        # kernel sweeps in the storage order of one strip); False where such strips are not taken at all
+        self.sweep = False
 
     def term(self, kind, dtype, pad0: int = 0, **kw) -> int:
         k = self.e.n_terms
@@ -378,6 +381,10 @@ class _Lowering:
             if self.size is None:
                 self.size, self.ctx = n.A.n, n.A.ctx
             strip = n.strip(self.part)
+            if strip is None and (self.sweep is None or self.sweep is n.A):
+                strip = n.strip(self.part, sweep=True)
+                if strip is not None:
+                    self.sweep = n.A
             if strip is not None:
                 # row i of A*x as a terminal: the row loop is generated into this expression's kernel (VEXB_TERM_SPMV)
                 xs = self.term(L.TERM_VEC, n.dtype, ptr=n.x.bufs[self.part].value or 0)
@@ -427,7 +434,7 @@ def _temporary(ctx, expr, n):
     """The expression evaluated into a vector of its own type (one extra pass): what a reduction folds when it cannot be
     served in one kernel."""
     tmp = vector(ctx, n, _VEXB2NP[expr.dtype])
-    tmp.assign(expr)
+    tmp._assign(L.SET, expr, sweep=False)
     return tmp
 
 
@@ -481,17 +488,20 @@ class InlineSpMV(Node):
         self.A, self.x, self.dtype = A, x, x.dtype
         self._tmp = None
 
-    def strip(self, part):
+    def strip(self, part, sweep=False):
+        """The strip of `part` as a terminal: thread per row (vexb_dspmat_inline_strip), or with sweep=True a sliced-ELL
+        strip for a storage-order sweep (vexb_dspmat_sweep_strip, assignments only)."""
         if not _is_float(self.dtype) or not hasattr(self.A, "parts"):
             return None
+        query = L.lib().vexb_dspmat_sweep_strip if sweep else L.lib().vexb_dspmat_inline_strip
         h = C.c_void_p()
-        L.check(L.lib().vexb_dspmat_inline_strip(self.A.parts[part], C.byref(h)))
+        L.check(query(self.A.parts[part], C.byref(h)))
         if not h.value:
             return None
         # all or nothing: an expression is lowered once per slot, and every slot must see the same kind of terminal
         for k in self.A.ctx.local:
             hk = C.c_void_p()
-            L.check(L.lib().vexb_dspmat_inline_strip(self.A.parts[k], C.byref(hk)))
+            L.check(query(self.A.parts[k], C.byref(hk)))
             if not hk.value:
                 return None
         return h.value
@@ -656,7 +666,7 @@ class vector(Node):
         return out[0]
 
     # -- assignment family (vector.hpp:666-801) ------------------------------------------------
-    def _assign(self, op: int, rhs):
+    def _assign(self, op: int, rhs, sweep=True):
         if isinstance(rhs, (SpMVTerm, Mixed)):
             return self._assign_mixed(op, Mixed.of(rhs))
         rhs = wrap(rhs)
@@ -664,6 +674,7 @@ class vector(Node):
         for k in self.ctx.local:
             low = _Lowering(k, self.part_start(k))
             low.size = self.n
+            low.sweep = None if sweep else False
             low.lower(rhs)
             L.check(lib.vexb_eval(self.ctx.devs[k], self.ctx.streams[k], self.bufs[k], self.dtype, op,
                                   C.byref(low.e), self.part_size(k), self.part_start(k)))
@@ -676,7 +687,8 @@ class vector(Node):
         # reads A and x once and writes y once.  Same operation order as the unfused path below for `=`.
         if (m.vec is not None or len(m.terms) > 1) and len(m.terms) <= 6 and _is_float(self.dtype) and getattr(self.ctx, "fuse_products", True):
             nodes = [InlineSpMV(t.A, t.x) if isinstance(t.A, SpMat) and isinstance(t.x, vector) and t.x.n == t.A.m else None for t in m.terms]
-            if all(nd is not None and nd.strip(self.ctx.local[0]) is not None for nd in nodes):
+            k0 = self.ctx.local[0]
+            if all(nd is not None and (nd.strip(k0) is not None or nd.strip(k0, sweep=True) is not None) for nd in nodes):
                 expr = m.vec
                 for t, nd in zip(m.terms, nodes):
                     prod = Binary("MUL", Scalar(float(t.scale), self.dtype), nd)

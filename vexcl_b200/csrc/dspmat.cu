@@ -238,6 +238,15 @@ extern "C" int vexb_dspmat_inline_strip(const vexb_dspmat *A, const vexb_spmat *
     return VEXB_OK;
 }
 
+extern "C" int vexb_dspmat_sweep_strip(const vexb_dspmat *A, const vexb_spmat **strip) {
+    VEXB_CHECK(A && strip, "NULL argument");
+    const vexb_spmat *S = A->loc;
+    const bool ok = S && !A->n_ghost && !A->bnd && !A->rem && !S->row_ids && S->y_offset == 0 && S->nrows_stored == A->nrows &&
+                    S->fmt == VEXB_FMT_SELL && !S->val_f32 && S->d_desc && param("spmv.sell_inline", 1) && !param("spmv.no_inline", 0);
+    *strip = ok ? S : nullptr;
+    return VEXB_OK;
+}
+
 extern "C" void *vexb_dspmat_send_buffer(const vexb_dspmat *A) { return A ? A->send_buf : nullptr; }
 extern "C" void *vexb_dspmat_ghost_buffer(const vexb_dspmat *A) { return A ? A->ghost_buf : nullptr; }
 

@@ -70,8 +70,25 @@ static const char *math_name(int op) {
 // buf_k rule (operations.hpp:2143-2157) and makes temporaries for `tie(x, y) = (x + y, y - x)` unnecessary.
 // The part shared by the elementwise and the reduction kernels: terminal table, user functions, sparse row functions and
 // one vexb_elem function per component (element i of the right-hand side, converted to the lhs type).
-static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtype, int aop, std::ostringstream &s, bool *spmv) {
+// A request whose products include a sliced-ELL strip is swept in that strip's storage order (generate_source_n), so it
+// holds at most one distinct such strip, any number of times.  *term: the first terminal on it, -1 when there is none.
+static int sell_sweep_term(const vexb_expr &e, int *term) {
+    *term = -1;
+    for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_SPMV) {
+        const vexb_spmat *A = static_cast<const vexb_spmat *>(e.term[k].v.ptr);
+        if (!A || A->fmt != VEXB_FMT_SELL) continue;
+        if (*term < 0) *term = k;
+        else if (e.term[*term].v.ptr != A) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "term %d: a second sliced-ELL strip in one expression (the kernel sweeps in the storage order of one)", k);
+    }
+    return VEXB_OK;
+}
+
+// sell: where the terminal of the request's sliced-ELL strip goes (sell_sweep_term); NULL for the callers that do not
+// sweep in storage order (reductions), which refuse such strips.
+static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtype, int aop, std::ostringstream &s, bool *spmv, int *sell = nullptr) {
     const vexb_expr &e = *es[0];
+    if (sell) VEXB_TRY(sell_sweep_term(e, sell));
+    const bool sweep = sell && *sell >= 0 && ncomp == 1;
     s << "// generated by libvexb200 (csrc/jit.cu)\n"
          "struct term_j { unsigned char kind, dtype, pad[6]; union { const void *ptr; double f64; float f32; int i32;"
          " unsigned int u32; long long i64; unsigned long long u64; } v; };\n"
@@ -99,19 +116,39 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
     for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_SPMV) {
         VEXB_CHECK(ncomp == 1, "sparse products are not fused into multi-expression kernels");
         const vexb_spmat *A = static_cast<const vexb_spmat *>(e.term[k].v.ptr);
-        VEXB_CHECK(A && (A->fmt == VEXB_FMT_CSR || A->fmt == VEXB_FMT_HELL) && !A->row_ids && A->y_offset == 0 && A->d_desc,
+        VEXB_CHECK(A && (A->fmt == VEXB_FMT_CSR || A->fmt == VEXB_FMT_HELL || (A->fmt == VEXB_FMT_SELL && sweep)) && !A->row_ids && A->y_offset == 0 && A->d_desc,
                    "term %d: this strip cannot be inlined into an expression (format / row map)", k);
         VEXB_CHECK(A->val_dtype == e.term[k].dtype, "term %d: value type of the matrix differs from the terminal's", k);
         VEXB_CHECK(!A->val_f32, "term %d: a strip with float values (VEXB_FMT_VALUES_F32) cannot be inlined into an expression", k);
         const char *T = ctype(e.term[k].dtype);
         if (!any_spmv) {
             s << "struct spmv_desc_j { const void *ell_col; const void *ell_val; const int *tail_ptr; const int *tail_col; const void *tail_val;\n"
-                 "                     const int *rowptr; const int *col; const void *val; unsigned long long pitch; int width; int shifts[" << kEllShiftSlots << "]; int x_max; };\n";
+                 "                     const int *rowptr; const int *col; const void *val; unsigned long long pitch; int width; int shifts[" << kEllShiftSlots << "]; int x_max;\n"
+                 "                     const int *slice_ptr; const int *perm; const void *sell_col; const void *sell_val; int sell_shift; unsigned long long n_slices; };\n";
             any_spmv = true;
         }
         s << "__device__ __forceinline__ " << T << " spmv_" << k << "(const spmv_desc_j *__restrict__ m, const " << T
-          << " *__restrict__ x, unsigned long long i) {\n  " << T << " sum = 0;\n";
-        if (A->fmt == VEXB_FMT_HELL) {
+          << " *__restrict__ x, unsigned long long i" << (A->fmt == VEXB_FMT_SELL ? ", unsigned long long t" : "") << ") {\n  " << T << " sum = 0;\n";
+        if (A->fmt == VEXB_FMT_SELL) {
+            // sell_kernel's loop for stored lane t (slice t >> 5, lane t & 31), which holds row i: 4 slots a turn -- their
+            // column and value loads, then the gathers -- then the remainder
+            const bool c16 = A->sell_col16 != nullptr;
+            const char *CT = c16 ? "short" : "int";
+            const char *dec = c16 ? "raw == (short)-32768 ? -1 : rs + (int)raw" : "raw";
+            s << "  const int base = __ldg(m->slice_ptr + (t >> 5)), w = (__ldg(m->slice_ptr + (t >> 5) + 1) - base) >> 5;\n"
+                 "  const " << CT << " *cp = (const " << CT << " *)m->sell_col + base + (t & 31);\n"
+                 "  const " << T << " *vp = (const " << T << " *)m->sell_val + base + (t & 31);\n";
+            if (c16) s << "  const int rs = (int)i + m->sell_shift;\n";
+            s << "  int k = 0;\n"
+                 "  for (; k + 4 <= w; k += 4) {\n"
+                 "    int c[4]; " << T << " v[4], xv[4];\n"
+                 "#pragma unroll\n    for (int u = 0; u < 4; ++u) { const " << CT << " raw = __ldcs(cp + (k + u) * 32); c[u] = " << dec << "; v[u] = __ldcs(vp + (k + u) * 32); }\n"
+                 "#pragma unroll\n    for (int u = 0; u < 4; ++u) xv[u] = c[u] != -1 ? __ldg(x + c[u]) : (" << T << ")0;\n"
+                 "#pragma unroll\n    for (int u = 0; u < 4; ++u) if (c[u] != -1) sum = sum + v[u] * xv[u];\n"
+                 "  }\n"
+                 "  for (; k < w; ++k) { const " << CT << " raw = __ldcs(cp + k * 32); const int c = " << dec << "; const " << T
+              << " v = __ldcs(vp + k * 32); if (c != -1) sum = sum + v * __ldg(x + c); }\n";
+        } else if (A->fmt == VEXB_FMT_HELL) {
             const int W = (int)A->ell_width;
             const bool c16 = A->ell_col16 != nullptr;
             const char *CT = c16 ? "short" : "int";
@@ -168,7 +205,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
     for (int comp = 0; comp < ncomp; ++comp) {
     const vexb_expr &e = *es[comp];
     s << "__device__ __forceinline__ " << LT << " vexb_elem" << (ncomp > 1 ? "_" + std::to_string(comp) : std::string()) << "(const terms_j &tt, const " << LT
-      << " *lhs, unsigned long long i, unsigned long long off) {\n";
+      << " *lhs, unsigned long long i, unsigned long long off" << (sweep ? ", unsigned long long t" : "") << ") {\n";
     std::vector<std::pair<std::string, int>> st;        // (variable name, dtype)
     for (int pc = 0; pc < e.n_code; ++pc) {
         const vexb_instr &in = e.code[pc];
@@ -183,7 +220,8 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
             if (tm.kind == VEXB_TERM_VEC) r << "__ldcs((const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr + i)";
             else if (tm.kind == VEXB_TERM_DSCALAR) r << "*(const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr";
             else if (tm.kind == VEXB_TERM_SPMV) r << "spmv_" << k << "((const spmv_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
-                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i)";
+                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i"
+                                                  << (static_cast<const vexb_spmat *>(tm.v.ptr)->fmt == VEXB_FMT_SELL ? ", t)" : ")");
             else if (tm.kind == VEXB_TERM_SCALAR) r << "tt.t[" << k << "].v." << ufield(rt);
             else r << "off + i + (unsigned long long)tt.t[" << k << "].v.i64";
         } else if (op == VEXB_OP_CVT) {
@@ -276,8 +314,25 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
 static int generate_source_n(const vexb_expr *const *es, int ncomp, int lhs_dtype, int aop, std::string *out) {
     std::ostringstream s;
     bool any_spmv = false;
-    VEXB_TRY(generate_elements(es, ncomp, lhs_dtype, aop, s, &any_spmv));
+    int sell = -1;
+    VEXB_TRY(generate_elements(es, ncomp, lhs_dtype, aop, s, &any_spmv, &sell));
     const char *LT = ctype(lhs_dtype);
+    if (sell >= 0) {
+        // Storage-order sweep: one thread per stored lane of the sliced-ELL strip, every operand and the target at the
+        // lane's row r.  A warp reads the strip's columns and values coalesced, as sell_kernel does, and its accesses to
+        // the other operands fall inside one window of sigma rows.  sell_layout puts every row in exactly one lane, so
+        // every element is written once.
+        s << "extern \"C\" __global__ void __launch_bounds__(256) vexb_jit_kernel(const terms_j tt, " << LT
+          << " *lhs, unsigned long long n, unsigned long long off) {\n"
+             "  const spmv_desc_j *m = (const spmv_desc_j *)tt.t[" << sell << "].v.ptr;\n"
+             "  const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;\n"
+             "  if (t >= m->n_slices * 32ull) return;\n"
+             "  const int r = __ldcs(m->perm + t);\n"
+             "  if (r < 0 || (unsigned long long)r >= n) return;\n"
+             "  lhs[r] = vexb_elem(tt, lhs, (unsigned long long)r, off, t);\n}\n";
+        *out = s.str();
+        return VEXB_OK;
+    }
     if (ncomp > 1) {
         s << "struct multi_j { terms_j c[" << ncomp << "]; " << LT << " *lhs[" << ncomp << "]; };\n"
              "extern \"C\" __global__ void __launch_bounds__(256) vexb_jit_kernel(const multi_j mt, unsigned long long n, unsigned long long off) {\n"
@@ -526,7 +581,7 @@ static std::string request_signature(const vexb_expr &e, int lhs_dtype, int aop)
         k.push_back((char)e.term[t].kind); k.push_back((char)e.term[t].dtype);
         if (e.term[t].kind == VEXB_TERM_SPMV) {          // the generated row loop depends on the strip's format, not on its data
             const vexb_spmat *A = static_cast<const vexb_spmat *>(e.term[t].v.ptr);
-            k.push_back((char)e.term[t].pad[0]); k.push_back((char)A->fmt); k.push_back(A->ell_class ? 3 : A->ell_mask ? 2 : A->ell_col16 ? 1 : 0); k.push_back(A->tail_nnz ? 1 : 0);
+            k.push_back((char)e.term[t].pad[0]); k.push_back((char)A->fmt); k.push_back(A->ell_class ? 3 : A->ell_mask ? 2 : A->ell_col16 || A->sell_col16 ? 1 : 0); k.push_back(A->tail_nnz ? 1 : 0);
             const unsigned w = (unsigned)A->ell_width;
             k.push_back((char)(w & 0xff)); k.push_back((char)((w >> 8) & 0xff)); k.push_back((char)((w >> 16) & 0xff)); k.push_back((char)(w >> 24));
         }
@@ -622,6 +677,8 @@ static void spawn_background(std::shared_ptr<JitEntry> en, const std::vector<vex
 int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const vexb_expr &e, size_t n, size_t index_offset,
              int mode, bool *done) {
     *done = false;
+    int sell = -1;
+    VEXB_TRY(sell_sweep_term(e, &sell));                              // before the cache: the signature does not tell strips apart
     std::shared_ptr<JitEntry> en;
     {
         std::lock_guard<std::mutex> lock(g_jmx);                      // short: map lookup only
@@ -681,6 +738,7 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     size_t blocks = (n + per_block - 1) / per_block;
     const size_t cap = (size_t)sm_count(dev) * 64;
     if (blocks > cap) blocks = cap;
+    if (sell >= 0) blocks = (static_cast<const vexb_spmat *>(e.term[sell].v.ptr)->n_slices + 7) / 8;   // a thread per stored lane, no loop
     CUresult r = g_jit.cuLaunchKernel(fn, (unsigned)blocks, 1, 1, 256, 1, 1, 0, (CUstream)st, args, nullptr);
     if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuLaunchKernel failed: %s", m); }
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -882,6 +940,8 @@ extern "C" int vexb_jit_precompile(int lhs_dtype, int assign_op, const vexb_expr
     VEXB_CHECK(assign_op >= VEXB_SET && assign_op <= VEXB_RSH, "bad assign op %d", assign_op);
     vexb_expr e;
     VEXB_TRY(normalize_expr(expr, &e, false));
+    int sell = -1;
+    VEXB_TRY(sell_sweep_term(e, &sell));
     VEXB_TRY(load_nvrtc());
     std::shared_ptr<JitEntry> en;
     {

@@ -76,6 +76,8 @@ struct SpmvDesc {
     const int *tail_ptr; const int *tail_col; const void *tail_val;
     const int *rowptr; const int *col; const void *val;
     unsigned long long pitch; int width; int shifts[kEllShiftSlots]; int x_max;
+    // sliced ELL: what sell_kernel takes (sell_col: 16-bit offsets when the strip has them, else 32-bit columns)
+    const int *slice_ptr; const int *perm; const void *sell_col; const void *sell_val; int sell_shift; unsigned long long n_slices;
 };
 }
 

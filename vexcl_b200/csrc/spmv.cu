@@ -963,6 +963,55 @@ __global__ void __launch_bounds__(256) sell_kernel(size_t n_slices, const int *_
     if (r >= 0) store_y<T>(y, row_ids ? (size_t)row_ids[r] : (size_t)r + y_offset, sum, alpha, append);
 }
 
+// K right-hand sides in one pass over a sliced-ELL strip (SpMat * multivector): sell_kernel's decomposition, a slot's
+// column and value loaded once and used for K gathers and K sums.  Per component the products are added in storage
+// order, as in sell_kernel on that component alone (same bits).
+template <class T, class C, int K>
+__global__ void __launch_bounds__(256) sell_multi_kernel(size_t n_slices, const int *__restrict__ slice_ptr, const int *__restrict__ perm,
+                                                         const C *__restrict__ col, int shift, const T *__restrict__ val,
+                                                         MultiPtr<K> mp, T alpha, int append,
+                                                         const int *__restrict__ row_ids, size_t y_offset) {
+    const size_t s = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (s >= n_slices) return;
+    const int lane = threadIdx.x & 31;
+    const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+    const int base = __ldg(slice_ptr + s), w = (__ldg(slice_ptr + s + 1) - base) >> 5;
+    const int r = ldg_stream(perm + s * 32 + lane, stream);
+    const C *cp = col + base + lane;
+    const T *vp = val + base + lane;
+    const size_t rr = r >= 0 ? (size_t)r : 0;
+    T sum[K];
+#pragma unroll
+    for (int q = 0; q < K; ++q) sum[q] = T(0);
+    int k = 0;
+    for (; k + 4 <= w; k += 4) {                          // 4 slots: 8 coalesced loads, then 4 K gathers
+        int c[4]; T v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) { c[u] = ell_column(ldg_stream(cp + (k + u) * 32, stream), rr, shift); v[u] = ldg_stream(vp + (k + u) * 32, stream); }
+        T xv[K][4];
+#pragma unroll
+        for (int q = 0; q < K; ++q)
+#pragma unroll
+            for (int u = 0; u < 4; ++u) xv[q][u] = c[u] != -1 ? ldg_keep(static_cast<const T *>(mp.x[q]) + c[u], keep) : T(0);
+#pragma unroll
+        for (int q = 0; q < K; ++q)
+#pragma unroll
+            for (int u = 0; u < 4; ++u) if (c[u] != -1) sum[q] = t_add<T>(sum[q], t_mul<T>(v[u], xv[q][u]));
+    }
+    for (; k < w; ++k) {
+        const int c = ell_column(ldg_stream(cp + k * 32, stream), rr, shift);
+        const T v = ldg_stream(vp + k * 32, stream);
+        if (c != -1) {
+#pragma unroll
+            for (int q = 0; q < K; ++q) sum[q] = t_add<T>(sum[q], t_mul<T>(v, ldg_keep(static_cast<const T *>(mp.x[q]) + c, keep)));
+        }
+    }
+    if (r < 0) return;
+    const size_t yr = row_ids ? (size_t)row_ids[r] : (size_t)r + y_offset;
+#pragma unroll
+    for (int q = 0; q < K; ++q) store_y<T>(static_cast<T *>(mp.y[q]), yr, sum[q], alpha, append);
+}
+
 template <class T>
 __global__ void zero_rows_kernel(T *y, size_t n, const int *__restrict__ row_ids) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1523,6 +1572,15 @@ static int spmv_multi_launch(const vexb_spmat *A, cudaStream_t st, const void *c
     const size_t n = A->nrows_stored;
     MultiPtr<K> mp;
     for (int k = 0; k < K; ++k) { mp.x[k] = x[k]; mp.y[k] = y[k]; }
+    if (A->fmt == VEXB_FMT_SELL) {
+        const unsigned sb = (unsigned)((A->n_slices + 7) / 8);
+        if (A->sell_col16) sell_multi_kernel<T, short, K><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col16, A->sell_shift,
+                                                                             (const T *)A->sell_val, mp, alpha, append, A->row_ids, A->y_offset);
+        else sell_multi_kernel<T, int, K><<<sb, 256, 0, st>>>(A->n_slices, A->sell_ptr, A->sell_perm, A->sell_col, 0,
+                                                             (const T *)A->sell_val, mp, alpha, append, A->row_ids, A->y_offset);
+        VEXB_LAUNCHED();
+        return VEXB_OK;
+    }
     const unsigned blocks = (unsigned)((n + 255) / 256);
 #define HM(W) do { \
         if (A->ell_col16) hell_multi_kernel<T, W, short, K><<<blocks, 256, 0, st>>>(n, A->ell_pitch, (int)A->ell_width, A->ell_col16, A->ell_shifts, \
@@ -1572,7 +1630,7 @@ int vexb::spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &
         std::vector<int> ids(*row_ids);
         st = upload(ids, 0, (void **)&A->row_ids, &A->device_bytes);
     }
-    if (st == VEXB_OK && (A->fmt == VEXB_FMT_CSR || A->fmt == VEXB_FMT_HELL)) {
+    if (st == VEXB_OK && (A->fmt == VEXB_FMT_CSR || A->fmt == VEXB_FMT_HELL || A->fmt == VEXB_FMT_SELL)) {
         SpmvDesc d; memset(&d, 0, sizeof(d));
         d.ell_col = A->ell_col_any(); d.ell_val = A->ell_val_any();
         d.tail_ptr = A->tail_ptr; d.tail_col = A->tail_col; d.tail_val = A->tail_val;
@@ -1580,6 +1638,8 @@ int vexb::spmat_from_csr(int dev, size_t nrows, size_t ncols, std::vector<int> &
         d.pitch = A->ell_pitch; d.width = (int)A->ell_width;
         for (int g = 0; g < kEllShiftSlots; ++g) d.shifts[g] = A->ell_shifts.s[g];
         d.x_max = A->ell_shifts.x_max;
+        d.slice_ptr = A->sell_ptr; d.perm = A->sell_perm; d.sell_val = A->sell_val; d.sell_shift = A->sell_shift; d.n_slices = A->n_slices;
+        d.sell_col = A->sell_col16 ? (const void *)A->sell_col16 : (const void *)A->sell_col;
         cudaError_t e = cudaMalloc(&A->d_desc, sizeof(d));
         if (e == cudaSuccess) e = cudaMemcpy(A->d_desc, &d, sizeof(d), cudaMemcpyHostToDevice);
         if (e != cudaSuccess) { set_error(__FILE__, __LINE__, "strip descriptor upload failed: %s", cudaGetErrorString(e)); st = VEXB_ERR_CUDA; }
@@ -1805,15 +1865,15 @@ extern "C" int vexb_spmv(int dev, void *stream, const vexb_spmat *A, const void 
     return spmv_launch<float>(A, (cudaStream_t)stream, (const float *)x, (float *)y, (float)alpha, append);
 }
 
-// y_k (=|+=) alpha * A x_k for k < nrhs, the matrix streamed once per group of up to 4 right-hand sides (hybrid-ELL
-// strips); other formats, float-valued strips (VEXB_FMT_VALUES_F32) and single vectors go through vexb_spmv one by one.
+// y_k (=|+=) alpha * A x_k for k < nrhs, the matrix streamed once per group of up to 4 right-hand sides (hybrid-ELL and
+// sliced-ELL strips); other formats, float-valued strips (VEXB_FMT_VALUES_F32) and single vectors go through vexb_spmv one by one.
 // vex::SpMat * vex::multivector.
 extern "C" int vexb_spmv_multi(int dev, void *stream, const vexb_spmat *A, int nrhs, const void *const *x, void *const *y,
                                double alpha, int append) {
     VEXB_CHECK(A && nrhs >= 1 && x && y, "bad arguments");
     VEXB_CHECK(dev == A->dev, "matrix lives on device %d, not %d", A->dev, dev);
     for (int k = 0; k < nrhs; ++k) VEXB_CHECK((A->nrows == 0 || y[k]) && (A->nnz == 0 || x[k]), "vector %d is NULL", k);
-    const bool fused = A->fmt == VEXB_FMT_HELL && !A->val_f32 && A->nnz > 0 && A->nrows_stored > 0 && nrhs > 1 && !param("spmv.no_multi", 0);
+    const bool fused = (A->fmt == VEXB_FMT_HELL || A->fmt == VEXB_FMT_SELL) && !A->val_f32 && A->nnz > 0 && A->nrows_stored > 0 && nrhs > 1 && !param("spmv.no_multi", 0);
     if (!fused) {
         for (int k = 0; k < nrhs; ++k) VEXB_TRY(vexb_spmv(dev, stream, A, x[k], y[k], alpha, append));
         return VEXB_OK;
