@@ -693,7 +693,9 @@ int vexb_dspmat_apply_multi(int nlocal, vexb_comm *const *comms, vexb_dspmat *co
 /* The product and a dot product with its result without re-reading the vectors: y (=|+=) alpha*A*x, and
  * d_result[k][0] = sum over all parts of dot_with . y (same bits on every GPU).  The product kernel leaves one partial
  * per block; a one-block second launch folds them and combines across the peer group.  With dot_with = x this is q = A*p, (p, q) of a CG iteration.  Needs the peer-memory halo on every part
- * (or a single part) and a hybrid-ELL interior strip; returns VEXB_ERR_UNSUPPORTED otherwise (compose apply + reduce). */
+ * (or a single part) and a hybrid-ELL or sliced-ELL (VEXB_FMT_SELL) interior strip with at least one entry and values
+ * of the vector type; returns VEXB_ERR_UNSUPPORTED otherwise (CSR or row-pattern interiors, VEXB_FMT_VALUES_F32,
+ * dspmat.no_peer_halo, dspmat.no_fused_dot: compose apply + reduce). */
 int vexb_dspmat_apply_dot(int nlocal, vexb_dspmat *const *parts, void *const *streams, const void *const *x,
                           void *const *y, double alpha, int append, const void *const *dot_with,
                           void *const *d_result, vexb_peer *const *peers);

@@ -988,7 +988,7 @@ class SpMat:
 def _spmat_apply_dot(self, x: "vector", y: "vector", out: "DeviceScalar", dot_with: Optional["vector"] = None,
                      alpha: float = 1.0, append: bool = False) -> bool:
     """y (=|+=) alpha*A*x and out = dot(dot_with or x, y) on every device.  The dot partials come out of the product kernel (plus a one-block fold launch) when the matrix has the
-    peer-memory halo (or a single part) and a hybrid-ELL interior (vexb_dspmat_apply_dot); otherwise the product followed
+    peer-memory halo (or a single part) and a hybrid- or sliced-ELL interior (vexb_dspmat_apply_dot); otherwise the product followed
     by a device-resident reduction.  Returns True when the fused kernel ran."""
     ctx, lib = self.ctx, L.lib()
     w = x if dot_with is None else dot_with

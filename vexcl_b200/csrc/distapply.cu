@@ -13,7 +13,8 @@
 //                        every neighbour's values for this epoch have landed, then  y = alpha*sum_local (+ y);
 //                        y += alpha*sum_remote  -- the order of csr.inl:188-209 (mul_local then mul_remote), so the bits
 //                        match the unfused path;
-//   blocks [P+B, ...)    interior rows (no ghost entries): the hybrid-ELL row body of hell_kernel, untouched by the halo.
+//   blocks [P+B, ...)    interior rows (no ghost entries): the hybrid-ELL row body of hell_kernel (a row per thread) or
+//                        the sliced-ELL body of sell_kernel (a slice per warp), untouched by the halo.
 //
 // Blocks are dispatched in index order: pushes leave first; the few boundary blocks come next and sit out the NVLink
 // round trip while the interior rows keep the SMs busy.  Ghost buffers and flags are double-buffered by epoch parity and protected by
@@ -70,6 +71,9 @@ struct DistArgs {
     // optional dot(dot_with, y_new)
     const T *dot_with; T *dot_result; void *dot_ws; PeerArgs pa;
     unsigned long long *fault_host;
+    // interior strip (sliced ELL): what sell_kernel takes; int_row_ids and y_off as above.  Last, so that the hybrid-ELL
+    // instantiations read every other field where they did before.
+    size_t n_slices; const int *sell_ptr, *sell_perm; const void *sell_col; const T *sell_val; int sell_shift;
 };
 
 template <class T> __device__ __forceinline__ T nan_of();
@@ -91,12 +95,63 @@ __device__ __forceinline__ bool wait_flag(const unsigned long long *flag, unsign
     }
 }
 
+// Column type of a sliced-ELL interior strip: dist_apply_kernel<T, 0, SellCol<C>, DOT> runs sell_kernel's body on it
+// (C = short: 16-bit offsets from (row + sell_shift), C = int: the columns).
+template <class C> struct SellCol {};
+template <class C> struct sell_col_of { using type = void; };
+template <class C> struct sell_col_of<SellCol<C>> { using type = C; };
+
+// Interior block ib of a sliced-ELL strip: 8 slices, one warp per slice and one lane per row, sell_kernel's loop
+// restated (4 slots a turn, then the rest one by one, products added in storage order, the same cache hints), so every
+// row gets the bits sell_kernel gives it.  Returns the lane's term of dot(dot_with, y_new); a padding lane (perm -1) and
+// a warp past the last slice write nothing and return +0, as a thread past the last row of the hybrid-ELL body does.
+template <class T, class C, bool DOT>
+__device__ __forceinline__ T dist_sell_rows(const DistArgs<T> &a, size_t ib) {
+    const size_t s = ib * 8 + (threadIdx.x >> 5);
+    if (s >= a.n_slices) return T(0);
+    const int lane = threadIdx.x & 31;
+    const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
+    const int base = __ldg(a.sell_ptr + s), w = (__ldg(a.sell_ptr + s + 1) - base) >> 5;
+    const int r = ldg_stream(a.sell_perm + s * 32 + lane, stream);
+    const C *cp = (const C *)a.sell_col + base + lane;
+    const T *vp = a.sell_val + base + lane;
+    const size_t rr = r >= 0 ? (size_t)r : 0;
+    T sum = T(0);
+    int k = 0;
+    for (; k + 4 <= w; k += 4) {
+        int c[4]; T v[4], xv[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) { c[u] = ell_column(ldg_stream(cp + (k + u) * 32, stream), rr, a.sell_shift); v[u] = ldg_stream(vp + (k + u) * 32, stream); }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) xv[u] = c[u] != -1 ? ldg_keep(a.x + c[u], keep) : T(0);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) if (c[u] != -1) sum = t_add<T>(sum, t_mul<T>(v[u], xv[u]));
+    }
+    for (; k < w; ++k) {
+        const int c = ell_column(ldg_stream(cp + k * 32, stream), rr, a.sell_shift);
+        const T v = ldg_stream(vp + k * 32, stream);
+        if (c != -1) sum = t_add<T>(sum, t_mul<T>(v, ldg_keep(a.x + c, keep)));
+    }
+    if (r < 0) return T(0);
+    const size_t ry = a.y_off + (a.int_row_ids ? (size_t)a.int_row_ids[r] : (size_t)r);
+    const T v = t_mul<T>(a.alpha, sum);
+    const T out = a.append ? t_add<T>(a.y[ry], v) : v;
+    a.y[ry] = out;
+    return DOT ? t_mul<T>(a.dot_with[ry], out) : T(0);
+}
+
 // dot partials: one value per block in dot_ws (own buffer, not the Reductor workspace)
 // Register bound: 32 per thread (8 blocks per SM).  Row-class strips get 40 (6 blocks per SM): under 32 their row body,
 // which keeps all W gathers of x in flight before the class byte returns (hell_class_rows), spilled 24 bytes at every
 // width, in the interior rows as well as the boundary rows.
+// C = SellCol<short | int>: the interior strip is sliced ELL (dist_sell_rows), W is 0.  In double those spilled 44 bytes
+// under 32 registers (4 slots of 8-byte values and gathers in flight beside the boundary rows' state) and get 40 (6 blocks
+// per SM) as well; in float they fit 32.
+template <class T, class C> constexpr int dist_min_blocks() {
+    return std::is_same<C, EllClass>::value || (!std::is_void<typename sell_col_of<C>::type>::value && sizeof(T) == 8) ? 6 : 8;
+}
 template <class T, int W, class C, bool DOT>
-__global__ void __launch_bounds__(256, std::is_same<C, EllClass>::value ? 6 : 8) dist_apply_kernel(const __grid_constant__ DistArgs<T> a) {
+__global__ void __launch_bounds__(256, dist_min_blocks<T, C>()) dist_apply_kernel(const __grid_constant__ DistArgs<T> a) {
     unsigned long long *mine = a.box[a.rank];
     __shared__ unsigned long long s_epoch;
     __shared__ int s_ok;
@@ -145,8 +200,11 @@ __global__ void __launch_bounds__(256, std::is_same<C, EllClass>::value ? 6 : 8)
         }
     } else if (b >= a.n_push_blocks + a.n_bnd_blocks) {
         // ---- interior rows ----
+        using SC = typename sell_col_of<C>::type;
         const size_t i = (size_t)(b - a.n_push_blocks - a.n_bnd_blocks) * blockDim.x + threadIdx.x;
-        if (i < a.n_int) {
+        if constexpr (!std::is_void<SC>::value) {
+            dot_acc = dist_sell_rows<T, SC, DOT>(a, (size_t)(b - a.n_push_blocks - a.n_bnd_blocks));
+        } else if (i < a.n_int) {
             const uint64_t stream = l2_policy_stream(), keep = l2_policy_keep();
             const T sum = hell_row_sum<T, W, C>(i, a.pitch, a.w_dyn, (const C *)a.ell_col, a.shift, a.ell_val, a.tail_ptr, a.tail_col,
                                                 a.tail_val, a.x, stream, keep);
@@ -448,10 +506,14 @@ template <class T, bool DOT>
 static int launch_dist(const vexb_dspmat *A, cudaStream_t st, const DistArgs<T> &a, unsigned grid) {
     const vexb_spmat *S = A->loc;
     const bool hell = S && S->fmt == VEXB_FMT_HELL && a.n_int_blocks > 0;
+    const bool sell = S && S->fmt == VEXB_FMT_SELL && a.n_int_blocks > 0;
     const size_t w = hell ? S->ell_width : 0;
 #define DL(W) do { if (hell && S->ell_col16) dist_apply_kernel<T, W, short, DOT><<<grid, 256, 0, st>>>(a); \
                    else dist_apply_kernel<T, W, int, DOT><<<grid, 256, 0, st>>>(a); } while (0)
-    if (hell && S->ell_class) {
+    if (sell) {
+        if (S->sell_col16) dist_apply_kernel<T, 0, SellCol<short>, DOT><<<grid, 256, 0, st>>>(a);
+        else dist_apply_kernel<T, 0, SellCol<int>, DOT><<<grid, 256, 0, st>>>(a);
+    } else if (hell && S->ell_class) {
         switch (w) {   // = the widths spmv.cu build() gives row classes
             case 5: dist_apply_kernel<T, 5, EllClass, DOT><<<grid, 256, 0, st>>>(a); break;
             case 7: dist_apply_kernel<T, 7, EllClass, DOT><<<grid, 256, 0, st>>>(a); break;
@@ -474,9 +536,10 @@ static int launch_dist(const vexb_dspmat *A, cudaStream_t st, const DistArgs<T> 
     return VEXB_OK;
 }
 
-// y (=|+=) alpha * A x for one part through the peer-memory halo.  If the interior strip is hybrid ELL everything is one
-// launch; otherwise the interior runs as its own kernel on `st` and push + boundary rows follow in a second launch on the
-// part's side stream (forked from / joined to `st` with events, so the pair is still graph-capturable).
+// y (=|+=) alpha * A x for one part through the peer-memory halo.  If the interior strip is hybrid or sliced ELL (with
+// entries) everything is one launch; otherwise the interior runs as its own kernel on `st` and push + boundary rows follow
+// in a second launch on the part's side stream (forked from / joined to `st` with events, so the pair is still
+// graph-capturable).
 template <class T>
 static int dist_apply_t(const vexb_dspmat *A, cudaStream_t st, const T *x, T *y, T alpha, int append, const T *dot_with,
                         T *dot_result, const vexb_peer *peer) {
@@ -499,15 +562,24 @@ static int dist_apply_t(const vexb_dspmat *A, cudaStream_t st, const T *x, T *y,
     if (peer && peer->nranks > 1) a.pa = peer->args();
     a.fault_host = h->fault_host;
     const vexb_spmat *S = A->loc;
-    const bool fused_interior = S && S->fmt == VEXB_FMT_HELL && S->nnz > 0 && S->nrows_stored > 0;
-    if (fused_interior) {
+    // an interior strip without entries keeps the second path: its product only zeroes y (spmv_launch)
+    const bool hell_interior = S && S->fmt == VEXB_FMT_HELL && S->nnz > 0 && S->nrows_stored > 0;
+    const bool sell_interior = S && S->fmt == VEXB_FMT_SELL && S->nnz > 0 && S->nrows_stored > 0;
+    const bool fused_interior = hell_interior || sell_interior;
+    if (hell_interior) {
         a.n_int = S->nrows_stored; a.pitch = S->ell_pitch; a.w_dyn = (int)S->ell_width; a.shift = S->ell_shifts;
         a.ell_col = S->ell_col_any(); a.ell_val = (const T *)S->ell_val_any();
         a.tail_ptr = S->tail_ptr; a.tail_col = S->tail_col; a.tail_val = (const T *)S->tail_val;
         a.int_row_ids = S->row_ids; a.y_off = S->y_offset;
         a.n_int_blocks = (int)((S->nrows_stored + 255) / 256);
+    } else if (sell_interior) {
+        a.n_slices = S->n_slices; a.sell_ptr = S->sell_ptr; a.sell_perm = S->sell_perm;
+        a.sell_col = S->sell_col16 ? (const void *)S->sell_col16 : (const void *)S->sell_col; a.sell_val = (const T *)S->sell_val;
+        a.sell_shift = S->sell_col16 ? S->sell_shift : 0;
+        a.int_row_ids = S->row_ids; a.y_off = S->y_offset;
+        a.n_int_blocks = (int)((S->n_slices + 7) / 8);                // 8 slices per block, as sell_kernel
     } else if (dot_with) {
-        VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "the fused product + dot needs a hybrid-ELL interior strip");
+        VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "the fused product + dot needs a hybrid- or sliced-ELL interior strip");
     }
     const unsigned grid = (unsigned)(a.n_push_blocks + a.n_int_blocks + a.n_bnd_blocks);
     if (dot_with) {

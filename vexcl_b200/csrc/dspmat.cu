@@ -385,7 +385,8 @@ extern "C" int vexb_dspmat_apply(int nlocal, vexb_comm *const *comms, vexb_dspma
 // fold that also combines across the GPUs of `peers` (every GPU ends with the same bits).  This is q = A p; (p, q) of a CG
 // iteration without re-reading p and q (the reference fuses the product into a consumer kernel on one device: sparse/product.hpp:45-130,
 // spmat/inline_spmv.hpp:68-76; its multi-device SpMat needs a separate reduction).  Needs the peer-memory halo on every
-// part (or a single part) and a hybrid-ELL interior strip: otherwise VEXB_ERR_UNSUPPORTED and the caller composes it.
+// part (or a single part) and a hybrid- or sliced-ELL interior strip with entries and values of the vector type: otherwise
+// VEXB_ERR_UNSUPPORTED and the caller composes it.
 extern "C" int vexb_dspmat_apply_dot(int nlocal, vexb_dspmat *const *parts, void *const *streams, const void *const *x,
                                      void *const *y, double alpha, int append, const void *const *dot_with,
                                      void *const *d_result, vexb_peer *const *peers) {
@@ -395,8 +396,9 @@ extern "C" int vexb_dspmat_apply_dot(int nlocal, vexb_dspmat *const *parts, void
         int c = 0;
         VEXB_TRY(vexb_dspmat_halo_connected(parts[k], &c));
         const vexb_spmat *S = parts[k]->loc;
-        if (!c || !S || S->fmt != VEXB_FMT_HELL || S->nnz == 0 || param("dspmat.no_peer_halo", 0) || param("dspmat.no_fused_dot", 0))
-            VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "fused product + dot needs the peer-memory halo and a hybrid-ELL interior strip on every part");
+        if (!c || !S || (S->fmt != VEXB_FMT_HELL && S->fmt != VEXB_FMT_SELL) || S->nnz == 0 || param("dspmat.no_peer_halo", 0) ||
+            param("dspmat.no_fused_dot", 0))
+            VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "fused product + dot needs the peer-memory halo and a hybrid- or sliced-ELL interior strip on every part");
         if (parts[k]->values_f32) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "no fused product + dot for float values (VEXB_FMT_VALUES_F32)");
         VEXB_CHECK(parts[k]->nparts == 1 || (peers && peers[k]), "part %d: a peer group is needed to combine the dot across GPUs", k);
     }

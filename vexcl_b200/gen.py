@@ -112,6 +112,26 @@ def irregular_rows(n: int, lo: int = 0, hi: int = 32, seed: int = 1, index_dtype
     return row.astype(index_dtype), col.astype(index_dtype), rng.random(nnz) - 0.5
 
 
+def irregular_spd(n: int, hi: int = 32, seed: int = 1, max_gap: int = 64):
+    """A symmetric positive definite matrix with irregular rows, for CG: the entries of irregular_rows(n, 0, hi, seed)
+    below the diagonal, without those clipping sent to column 0 (they would pile up in row 0 and give the spectrum an
+    outlier) and one per column where clipping repeated a column, mirrored above the diagonal; on the diagonal 1 + the
+    row's sum of |off-diagonal| (strictly diagonally dominant).  Rows hold 1 to about hi entries, about hi / 2 on average.
+    Returns int64 row, col and float64 val, columns ascending."""
+    row, col, val = irregular_rows(n, 0, hi, seed, np.int64, max_gap)
+    r = np.repeat(np.arange(n, dtype=np.int64), np.diff(row))
+    low = (col < r) & (col > 0)
+    _, first = np.unique(r[low] * n + col[low], return_index=True)
+    i, j, v = r[low][first], col[low][first], val[low][first]
+    d = np.arange(n, dtype=np.int64)
+    rr, cc = np.concatenate([i, j, d]), np.concatenate([j, i, d])
+    vv = np.concatenate([v, v, 1.0 + np.bincount(i, np.abs(v), n) + np.bincount(j, np.abs(v), n)])
+    order = np.argsort(rr * n + cc, kind="stable")
+    out = np.zeros(n + 1, np.int64)
+    np.cumsum(np.bincount(rr, minlength=n), out=out[1:])
+    return out, cc[order], vv[order]
+
+
 def ccsr_bytes(nrows: int, idx_bytes: int = 8) -> int:
     """Algorithmic bytes of y = A*x for a CCSR matrix: idx as the reference stores it (size_t), x and y once; the
     unique-row table is negligible."""

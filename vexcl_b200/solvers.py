@@ -93,7 +93,10 @@ class CGFused:
 
     against 7 vector kernels + 3 scalar kernels (+ pack, NCCL, boundary kernels) for CGDevice: 64 instead of 96 bytes
     of vector traffic per row and iteration besides the product.  rho and rho' swap roles every iteration (no copy),
-    so two CUDA graphs (even / odd) replay the solver.  Per-element arithmetic is the unfused composition's."""
+    so two CUDA graphs (even / odd) replay the solver.  Per-element arithmetic is the unfused composition's.
+    The product step is fused on matrices whose interior strips are hybrid ELL or sliced ELL (VEXB_FMT_AUTO's choice for
+    uneven rows); on CSR or float-valued strips, and on several slots without a peer group, apply_dot composes the
+    product and a reduction (fused_product is then False)."""
 
     def __init__(self, A: SpMat, b: vector, x: vector):
         ctx = self.ctx = A.ctx
