@@ -106,7 +106,7 @@ typedef enum {
     VEXB_TERM_INDEX = 2,  /* element_index: index_offset + i + v.i64 (element_index.hpp:40-111), type u64 */
     VEXB_TERM_DSCALAR = 3,/* v.ptr: ONE device-resident value of `dtype`, broadcast to every element.  Lets the
                              result of vexb_reduce feed the next expression without a host round trip. */
-    VEXB_TERM_SPMV = 4    /* v.ptr: a vexb_spmat (host handle; CSR or hybrid ELL, plain strip -- or, in vexb_eval only,
+    VEXB_TERM_SPMV = 4,   /* v.ptr: a vexb_spmat (host handle; CSR or hybrid ELL, plain strip -- or, in vexb_eval only,
                              sliced ELL: see vexb_dspmat_sweep_strip); pad[0]: slot of the
                              VEXB_TERM_VEC holding x.  Element i evaluates to row i of A*x (products added in storage
                              order, as vexb_spmv does): the sparse product as a *terminal* of the consumer's kernel --
@@ -115,6 +115,21 @@ typedef enum {
                              spmat/inline_spmv.hpp:68-76).  Expressions with such terminals run on the NVRTC side path
                              (the row loop is generated into the kernel, specialised to the strip's format and width),
                              reductions of them included (vexb_reduce_all / vexb_reduce_multi). */
+    VEXB_TERM_CCSR = 5    /* v.ptr: a vexb_ccsr (host handle); pad[0]: slot of the VEXB_TERM_VEC holding x; pad[1]: the
+                             matrix's idx width on the device (vexb_ccsr_info.idx_bytes: 1, 2 or 4); dtype: the matrix's
+                             value type, which is also x's.  Element i evaluates to
+                                 s = 0;  s = s + val[j] * x[i + col[j]]  for j over the unique row idx[i], in storage order,
+                             every product and sum rounded on its own: the bits of vexb_ccsr_spmv(alpha = 1, append = 0) at
+                             row i -- the reference's ccsr_product terminal (spmat/ccsr.hpp:88-270), `sin(A*x)`,
+                             `x * (A*x)`, `sum(x * (A*x))` in one launch.  Served like VEXB_TERM_SPMV by the NVRTC kernels of
+                             vexb_eval, vexb_reduce_all and vexb_reduce_multi (one kernel per value type and idx width, not per
+                             matrix: the row loop reads the unique-row table through a small device descriptor that the
+                             handle allocates, with a blocking copy, at its first use as a terminal); vexb_eval_multi reports
+                             it as not handled.  Checked before any launch (VEXB_ERR_INVALID otherwise): the handle lives on
+                             `dev`, dtype is its value type, the call covers the whole matrix (index_offset 0, n = nrows),
+                             pad[0] names a vector terminal of that type, pad[1] agrees with the handle.  vexb_eval returns
+                             VEXB_ERR_UNSUPPORTED when x is the assignment's target (threads would write x[i] while others
+                             read x[i + col[j]]): evaluate the product into a temporary first. */
 } vexb_term_kind;
 
 typedef struct {

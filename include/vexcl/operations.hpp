@@ -29,7 +29,9 @@ template <typename T> class vector;
 
 /// Marker base of every expression node and terminal.
 struct vector_expr_tag {};
-template <class T> struct is_vector_expr : std::is_base_of<vector_expr_tag, typename std::decay<T>::type> {};
+/// Specialised for operands that are not nodes: vex::SpMatCCSR products (spmat/ccsr.hpp).
+template <class T> struct is_vector_expr_type : std::is_base_of<vector_expr_tag, T> {};
+template <class T> struct is_vector_expr : is_vector_expr_type<typename std::decay<T>::type> {};
 
 /// Assignment operators, same set as vexcl/operations.hpp:70-80.
 namespace assign {
@@ -88,6 +90,15 @@ struct ir_builder {
         e.term[k].pad[0] = static_cast<uint8_t>(xs);
         emit(VEXB_OP_TERM, dtype, k);
     }
+    /// Row `i` of `A * x` for a vex::SpMatCCSR (VEXB_TERM_CCSR); idx_bytes: the matrix's idx width on the device.
+    void push_ccsr(const vexb_ccsr *A, int idx_bytes, const void *xptr, int dtype) {
+        int xs = new_term();
+        e.term[xs].kind = VEXB_TERM_VEC; e.term[xs].dtype = static_cast<uint8_t>(dtype); e.term[xs].v.ptr = xptr;
+        int k = new_term();
+        e.term[k].kind = VEXB_TERM_CCSR; e.term[k].dtype = static_cast<uint8_t>(dtype); e.term[k].v.ptr = A;
+        e.term[k].pad[0] = static_cast<uint8_t>(xs); e.term[k].pad[1] = static_cast<uint8_t>(idx_bytes);
+        emit(VEXB_OP_TERM, dtype, k);
+    }
     void cvt(int from, int to) { if (from != to) emit(VEXB_OP_CVT, to, from); }
 };
 
@@ -98,6 +109,7 @@ struct expr_props {
     size_t size = 0;
     bool sized = false;
     int comp = -1;                  ///< component being prepared (multi-expressions), else -1
+    const void *target = nullptr;   ///< assignments: device slice 0 of the left-hand side (a CCSR product of it takes a temporary)
     /// Assignments only (assign_expression): the generated kernel may sweep in the storage order of ONE sliced-ELL strip
     /// (vexb_dspmat_sweep_strip).  The first product that asks claims it; products of other such matrices take a temporary.
     bool sweeps = false;
@@ -509,6 +521,7 @@ void assign_expression(vex::vector<T> &lhs, const Expr &expr, int comp = -1) {
     expr_props p;
     p.comp = comp;
     p.sweeps = comp < 0;
+    if (lhs.nparts()) p.target = lhs(0).raw();
     p.see(lhs.queue_list(), lhs.partition(), lhs.size());
     expr.props(p);
     const std::vector<backend::command_queue> &queue = lhs.queue_list();

@@ -124,7 +124,7 @@ class Reductor {
 
         template <class Expr>
         typename std::enable_if<is_vector_expr<Expr>::value && detail::ncomp<Expr>::value == 0, result_type>::type
-        operator()(const Expr &expr) const { return reduce(expr, -1); }
+        operator()(const Expr &expr) const { return reduce(detail::operand<Expr>::wrap(expr), -1); }
 
         /// Multi-expressions reduce component by component (reductor.hpp:341-349).
         template <class Expr>

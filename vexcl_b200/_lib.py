@@ -16,7 +16,7 @@ ERR_CUDA, ERR_INVALID, ERR_NCCL, ERR_UNSUPPORTED, ERR_NOMEM, ERR_PEER = range(1,
 F64, F32, I32, U32, I64, U64 = range(6)
 SET, ADD, SUB, MUL, DIV, MOD, AND, OR, XOR, LSH, RSH = range(11)
 SUM, SUM_KAHAN, MAX, MIN, MINMAX = range(5)
-TERM_VEC, TERM_SCALAR, TERM_INDEX, TERM_DSCALAR, TERM_SPMV = range(5)
+TERM_VEC, TERM_SCALAR, TERM_INDEX, TERM_DSCALAR, TERM_SPMV, TERM_CCSR = range(6)
 FMT_AUTO, FMT_CSR, FMT_HELL, FMT_PATTERNS, FMT_SELL = range(5)
 FMT_VALUES_F32 = 0x100          # ORed into fmt: double values stored as float, double vectors and sums
 MAX_TERMS, MAX_CODE, MAX_STACK = 16, 64, 12

@@ -333,6 +333,8 @@ pow_, atan2, fmod, hypot, fmin, fmax, fma = (_mkfunc(o) for o in ("POW", "ATAN2"
 def wrap(x) -> Node:
     if isinstance(x, Node):
         return x
+    if isinstance(x, SpMVTerm) and isinstance(x.A, SpMatCCSR) and isinstance(x.x, vector):
+        return CcsrProduct(x.A, x.x, x.scale)                  # a CCSR product where an operand goes
     return Scalar(x)
 
 
@@ -345,6 +347,10 @@ class _Lowering:
         # assignments only: the one matrix whose sliced-ELL strips this expression may take as terminals (the generated
         # kernel sweeps in the storage order of one strip); False where such strips are not taken at all
         self.sweep = False
+        # assignments only: the target vector; a CCSR product of it is evaluated into a temporary (kept here until the
+        # launch is enqueued)
+        self.target = None
+        self.keep = []
 
     def term(self, kind, dtype, pad0: int = 0, **kw) -> int:
         k = self.e.n_terms
@@ -391,6 +397,23 @@ class _Lowering:
                 self.emit("TERM", n.dtype, self.term(L.TERM_SPMV, n.dtype, pad0=xs, ptr=strip))
             else:
                 self.lower(n.temporary())
+        elif isinstance(n, CcsrProduct):
+            if self.size is None:
+                self.size, self.ctx = n.A.n, n.A.ctx
+            if n.scale != 1.0:
+                self.lower(Scalar(n.scale, n.dtype))
+            if n.x is self.target:
+                tmp = n.temporary()                     # x[i] written while other threads read x[i + col[j]] would race
+                self.keep.append(tmp)
+                self.lower(tmp)
+            else:
+                # row i of A*x as a terminal: the CCSR row loop is generated into this expression's kernel (VEXB_TERM_CCSR)
+                xs = self.term(L.TERM_VEC, n.dtype, ptr=n.x.bufs[self.part].value or 0)
+                k = self.term(L.TERM_CCSR, n.dtype, pad0=xs, ptr=n.A.h.value)
+                self.e.term[k].pad[1] = n.A.idx_bytes
+                self.emit("TERM", n.dtype, k)
+            if n.scale != 1.0:
+                self.emit("MUL", n.dtype)
         elif isinstance(n, Scalar):
             field = {L.F64: "f64", L.F32: "f32", L.I32: "i32", L.U32: "u32", L.I64: "i64", L.U64: "u64"}[n.dtype]
             self.emit("TERM", n.dtype, self.term(L.TERM_SCALAR, n.dtype, **{field: n.value}))
@@ -424,7 +447,7 @@ class _Lowering:
 
 
 def _has_call(n) -> bool:
-    if isinstance(n, (Call, InlineSpMV)):
+    if isinstance(n, (Call, InlineSpMV, CcsrProduct)):
         return True
     kids = [getattr(n, c, None) for c in ("a", "b", "cond")] + list(getattr(n, "args", []))
     return any(isinstance(k, Node) and _has_call(k) for k in kids)
@@ -460,7 +483,7 @@ def _find_props(n: Node):
     """(ctx, size) of the first vector terminal (get_expression_properties, operations.hpp:1411)."""
     if isinstance(n, vector):
         return n.ctx, n.n
-    if isinstance(n, InlineSpMV):
+    if isinstance(n, (InlineSpMV, CcsrProduct)):
         return n.A.ctx, n.A.n
     for child in ("a", "b", "cond"):
         c = getattr(n, child, None)
@@ -517,7 +540,29 @@ def make_inline(term):
     """vex::make_inline(A * x): the (unscaled) product as an expression terminal."""
     if not isinstance(term, SpMVTerm) or term.scale != 1.0:
         raise ValueError("make_inline: scale the inlined product inside the expression instead")
+    if isinstance(term.A, SpMatCCSR):
+        return CcsrProduct(term.A, term.x)
     return InlineSpMV(term.A, term.x)
+
+
+class CcsrProduct(Node):
+    """`A * x` of a SpMatCCSR where an operand goes -- vx.sin(A * x), x * (A * x), y *= A * x, user function arguments,
+    if_else, Reductor calls, make_inline(A * x): the reference's ccsr_product terminal (spmat/ccsr.hpp:88-270).  Lowered
+    to VEXB_TERM_CCSR, whose row loop is generated into the consumer's kernel (same bits as a temporary from A.apply),
+    scaled inside the expression when it carries a scale.  When x is the assignment's target the product is evaluated
+    into a temporary first."""
+
+    def __init__(self, A, x, scale=1.0):
+        if x.n != A.n:
+            raise ValueError("SpMatCCSR product: vector size does not match the matrix")
+        if x.dtype != A.val_dtype:
+            raise TypeError("SpMatCCSR product: the vector's type differs from the matrix's value type")
+        self.A, self.x, self.scale, self.dtype = A, x, scale, A.val_dtype
+
+    def temporary(self):
+        tmp = vector(self.A.ctx, self.A.n, self.x.np_dtype)
+        self.A.apply(self.x, tmp, 1.0, False)
+        return tmp
 
 
 # ------------------------------------------------------------------------------------------- SpMV additive terms
@@ -527,10 +572,24 @@ class SpMVTerm:
     def __init__(self, A, x, scale=1.0):
         self.A, self.x, self.scale = A, x, scale
 
-    def __mul__(self, s): return SpMVTerm(self.A, self.x, self.scale * s)
-    __rmul__ = __mul__
-    def __truediv__(self, s): return SpMVTerm(self.A, self.x, self.scale / s)
+    def _operand(self, o):
+        """A CCSR product meeting another expression (not a scale) becomes an operand: CcsrProduct."""
+        return isinstance(self.A, SpMatCCSR) and isinstance(o, (Node, SpMVTerm))
+
+    def __mul__(self, s): return wrap(self) * s if self._operand(s) else SpMVTerm(self.A, self.x, self.scale * s)
+    def __rmul__(self, s): return s * wrap(self) if self._operand(s) else SpMVTerm(self.A, self.x, self.scale * s)
+    def __truediv__(self, s): return wrap(self) / s if self._operand(s) else SpMVTerm(self.A, self.x, self.scale / s)
     def __neg__(self): return SpMVTerm(self.A, self.x, -self.scale)
+
+    def _cmp(self, op, o):
+        if not isinstance(self.A, SpMatCCSR):
+            return NotImplemented
+        return Node._bin(wrap(self), op, o)
+
+    def __lt__(self, o): return self._cmp("LT", o)
+    def __gt__(self, o): return self._cmp("GT", o)
+    def __le__(self, o): return self._cmp("LE", o)
+    def __ge__(self, o): return self._cmp("GE", o)
     def __add__(self, o): return Mixed(None, [self]) + o
     def __radd__(self, o): return Mixed(None, [self]).__radd__(o)
     def __sub__(self, o): return Mixed(None, [self]) - o
@@ -667,6 +726,8 @@ class vector(Node):
 
     # -- assignment family (vector.hpp:666-801) ------------------------------------------------
     def _assign(self, op: int, rhs, sweep=True):
+        if isinstance(rhs, SpMVTerm) and isinstance(rhs.A, SpMatCCSR) and op not in (L.SET, L.ADD, L.SUB):
+            rhs = wrap(rhs)                 # y *= A*x: the product as an operand; =, += and -= keep the additive path
         if isinstance(rhs, (SpMVTerm, Mixed)):
             return self._assign_mixed(op, Mixed.of(rhs))
         rhs = wrap(rhs)
@@ -674,6 +735,7 @@ class vector(Node):
         for k in self.ctx.local:
             low = _Lowering(k, self.part_start(k))
             low.size = self.n
+            low.target = self
             low.sweep = None if sweep else False
             low.lower(rhs)
             L.check(lib.vexb_eval(self.ctx.devs[k], self.ctx.streams[k], self.bufs[k], self.dtype, op,
@@ -1050,6 +1112,7 @@ class SpMatCCSR:
         L.check(L.lib().vexb_ccsr_create(ctx.devs[k], ctx.streams[k], self.n, self.m, _ip(idx), idx.dtype.itemsize,
                                          _ip(row), row.dtype.itemsize, _ip(col), col.dtype.itemsize, _ip(val),
                                          self.val_dtype, C.byref(self.h)))
+        self.idx_bytes = self.info().idx_bytes              # width of idx on the device: part of a terminal's kernel shape
 
     def __del__(self):
         try:

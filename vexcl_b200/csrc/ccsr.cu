@@ -13,6 +13,7 @@
 // Products and sums are rounded separately and accumulated in storage order (no FMA), so the result is
 // bit-identical to the reference's loop compiled without contraction (oracle/ccsr.py).
 #include <algorithm>
+#include <mutex>
 #include <string>
 #include <vector>
 #include "common.cuh"
@@ -26,6 +27,7 @@ struct vexb_ccsr {
     bool table_in_smem = true;
     std::vector<int> hrow, hcol; std::vector<double> hval;    // host copy of the unique-row table (source of the specialised kernel)
     void *jit_fn = nullptr; bool jit_failed = false;
+    void *term_desc = nullptr;                                 // {idx, row, col, val} in device memory, for VEXB_TERM_CCSR
 };
 
 namespace vexb {
@@ -390,8 +392,34 @@ extern "C" int vexb_ccsr_destroy(vexb_ccsr *A) {
     if (!A) return VEXB_OK;
     VEXB_RELEASE_GUARD();
     DeviceGuard g(A->dev);
-    cudaFree(A->idx); cudaFree(A->row); cudaFree(A->col); cudaFree(A->val);
+    cudaFree(A->idx); cudaFree(A->row); cudaFree(A->col); cudaFree(A->val); cudaFree(A->term_desc);
     delete A;
+    return VEXB_OK;
+}
+
+int vexb::ccsr_term_check(const vexb_ccsr *A, int k, int dev, int dtype, int idx_bytes, size_t n, size_t index_offset) {
+    VEXB_CHECK(A->dev == dev, "term %d: the CCSR matrix lives on device %d, not %d", k, A->dev, dev);
+    VEXB_CHECK(A->val_dtype == dtype, "term %d: the CCSR matrix holds values of type %d, the terminal says %d", k, A->val_dtype, dtype);
+    VEXB_CHECK(idx_bytes == A->idx_bytes, "term %d: the CCSR matrix stores idx in %d bytes, the terminal says %d", k, A->idx_bytes, idx_bytes);
+    VEXB_CHECK(index_offset == 0 && n == A->n, "term %d: a CCSR product covers the whole matrix (%zu rows), not elements [%zu, %zu)",
+               k, A->n, index_offset, index_offset + n);
+    return VEXB_OK;
+}
+
+int vexb::ccsr_term_desc(const vexb_ccsr *A, void **desc) {
+    static std::mutex mx;
+    std::lock_guard<std::mutex> lock(mx);
+    vexb_ccsr *M = const_cast<vexb_ccsr *>(A);                       // lazily attaches the descriptor
+    if (!M->term_desc) {
+        const void *h[4] = {A->idx, A->row, A->col, A->val};
+        DeviceGuard g(A->dev); VEXB_CHECK(g.ok, "cannot select device %d", A->dev);
+        void *d = nullptr;
+        VEXB_CUDA(cudaMalloc(&d, sizeof(h)));
+        const cudaError_t e = cudaMemcpy(d, h, sizeof(h), cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { cudaFree(d); VEXB_FAIL(VEXB_ERR_CUDA, "CCSR terminal descriptor: %s", cudaGetErrorString(e)); }
+        M->term_desc = d;
+    }
+    *desc = M->term_desc;
     return VEXB_OK;
 }
 

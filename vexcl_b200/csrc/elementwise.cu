@@ -188,7 +188,7 @@ extern "C" int vexb_eval_path(int lhs_dtype, int assign_op, const vexb_expr *exp
     ShapeMatch m; SweepArgs a;
     // alignment is checked on the real pointers too: a 32-byte aligned dummy lhs stands in here
     alignas(32) static char dummy[32];
-    if (expr_has_call(e) || expr_has_spmv(e)) snprintf(buf, buflen, "jit");
+    if (expr_has_call(e) || expr_has_product(e)) snprintf(buf, buflen, "jit");
     else if (plan_sweep(dummy, lhs_dtype, assign_op, e, &m, &a)) snprintf(buf, buflen, "sweep:%s", shape_name(m.shape));
     else snprintf(buf, buflen, param("eval.jit", 0) == 1 ? "jit" : "interp");
     return VEXB_OK;
@@ -208,7 +208,7 @@ extern "C" int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int as
 
     // user functions have no pre-compiled form: NVRTC side path (csrc/jit.cu)
     // ... and neither have sparse products used as terminals: their row loops are generated into the kernel
-    if (expr_has_call(e) || expr_has_spmv(e)) { bool done = false; return jit_eval(dev, st, lhs, lhs_dtype, assign_op, e, n, index_offset, 1, &done); }
+    if (expr_has_call(e) || expr_has_product(e)) { bool done = false; return jit_eval(dev, st, lhs, lhs_dtype, assign_op, e, n, index_offset, 1, &done); }
 
     ShapeMatch m; SweepArgs a;
     if (plan_sweep(lhs, lhs_dtype, assign_op, e, &m, &a)) {

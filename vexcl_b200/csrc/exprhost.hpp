@@ -72,8 +72,11 @@ inline void convert_scalar_term(vexb_term &t, int to) {
     t.dtype = (uint8_t)to;
 }
 
-inline bool expr_has_spmv(const vexb_expr &e) {
-    for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_SPMV) return true;
+inline bool is_product_term(int kind) { return kind == VEXB_TERM_SPMV || kind == VEXB_TERM_CCSR; }
+
+// Sparse products used as terminals (VEXB_TERM_SPMV, VEXB_TERM_CCSR): their row loops are generated into the kernel.
+inline bool expr_has_product(const vexb_expr &e) {
+    for (int k = 0; k < e.n_terms; ++k) if (is_product_term(e.term[k].kind)) return true;
     return false;
 }
 
@@ -100,13 +103,21 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     VEXB_CHECK(in->n_code >= 1 && in->n_code <= VEXB_MAX_CODE, "n_code=%d out of range", in->n_code);
     for (int k = 0; k < in->n_terms; ++k) {
         const vexb_term &t = in->term[k];
-        VEXB_CHECK(t.kind <= VEXB_TERM_SPMV, "term %d: bad kind %d", k, (int)t.kind);
+        VEXB_CHECK(t.kind <= VEXB_TERM_CCSR, "term %d: bad kind %d", k, (int)t.kind);
         VEXB_CHECK(t.dtype <= VEXB_U64, "term %d: bad dtype %d", k, (int)t.dtype);
         VEXB_CHECK(!need_ptrs || (t.kind != VEXB_TERM_VEC && t.kind != VEXB_TERM_DSCALAR) || t.v.ptr != nullptr, "term %d: NULL device pointer", k);
         if (t.kind == VEXB_TERM_SPMV) {
             VEXB_CHECK(t.v.ptr != nullptr, "term %d: NULL matrix handle", k);
             VEXB_CHECK(t.pad[0] < in->n_terms && in->term[t.pad[0]].kind == VEXB_TERM_VEC && in->term[t.pad[0]].dtype == t.dtype,
                        "term %d: the sparse product's x must be a vector terminal of the matrix's value type", k);
+        }
+        if (t.kind == VEXB_TERM_CCSR) {
+            // the handle is not read here: a source query (vexb_jit_source*) may pass NULL with pad[1] set
+            VEXB_CHECK(!need_ptrs || t.v.ptr != nullptr, "term %d: NULL CCSR matrix handle", k);
+            VEXB_CHECK(t.dtype == VEXB_F64 || t.dtype == VEXB_F32, "term %d: CCSR values are float or double", k);
+            VEXB_CHECK(t.pad[1] == 1 || t.pad[1] == 2 || t.pad[1] == 4, "term %d: CCSR idx width %d is not 1, 2 or 4", k, (int)t.pad[1]);
+            VEXB_CHECK(t.pad[0] < in->n_terms && in->term[t.pad[0]].kind == VEXB_TERM_VEC && in->term[t.pad[0]].dtype == t.dtype,
+                       "term %d: the CCSR product's x must be a vector terminal of the matrix's value type", k);
         }
     }
     // 1. de-duplicate vector terminals (same pointer, same dtype) and drop unused ones.
@@ -133,7 +144,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
                 for (int j = 0; j < out->n_terms; ++j)
                     if (out->term[j].kind == t.kind && out->term[j].v.ptr == t.v.ptr && out->term[j].dtype == t.dtype) { slot = j; break; }
             }
-            if (slot < 0 && t.kind == VEXB_TERM_SPMV) {
+            if (slot < 0 && is_product_term(t.kind)) {
                 // the x it multiplies: an ordinary vector terminal (shared with other uses of the same vector)
                 const vexb_term &xt = in->term[t.pad[0]];
                 int xs = remap[t.pad[0]];
@@ -142,11 +153,13 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
                 if (xs < 0) { VEXB_CHECK(out->n_terms < VEXB_MAX_TERMS, "too many terminals"); xs = out->n_terms++; out->term[xs] = xt; memset(out->term[xs].pad, 0, sizeof(xt.pad)); }
                 remap[t.pad[0]] = xs;
                 for (int j = 0; j < out->n_terms; ++j)
-                    if (out->term[j].kind == VEXB_TERM_SPMV && out->term[j].v.ptr == t.v.ptr && out->term[j].pad[0] == xs) { slot = j; break; }
+                    if (out->term[j].kind == t.kind && out->term[j].v.ptr == t.v.ptr && out->term[j].pad[0] == xs &&
+                        (t.kind != VEXB_TERM_CCSR || out->term[j].pad[1] == t.pad[1])) { slot = j; break; }
                 if (slot < 0) {
                     VEXB_CHECK(out->n_terms < VEXB_MAX_TERMS, "too many terminals");
                     slot = out->n_terms++; out->term[slot] = t; memset(out->term[slot].pad, 0, sizeof(t.pad));
                     out->term[slot].pad[0] = (uint8_t)xs;
+                    if (t.kind == VEXB_TERM_CCSR) out->term[slot].pad[1] = t.pad[1];      // idx width
                 }
             }
             if (slot < 0) { slot = out->n_terms++; out->term[slot] = t; memset(out->term[slot].pad, 0, sizeof(t.pad)); }
@@ -197,10 +210,10 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     // 3. compact away scalar slots orphaned by folding
     bool used[VEXB_MAX_TERMS] = {false};
     for (int pc = 0; pc < out->n_code; ++pc) if (out->code[pc].op == VEXB_OP_TERM) used[out->code[pc].arg] = true;
-    for (int k = 0; k < out->n_terms; ++k) if (used[k] && out->term[k].kind == VEXB_TERM_SPMV) used[out->term[k].pad[0]] = true;
+    for (int k = 0; k < out->n_terms; ++k) if (used[k] && is_product_term(out->term[k].kind)) used[out->term[k].pad[0]] = true;
     int newslot[VEXB_MAX_TERMS]; int n = 0;
     for (int k = 0; k < out->n_terms; ++k) newslot[k] = used[k] ? n++ : -1;
-    for (int k = 0; k < out->n_terms; ++k) if (used[k] && out->term[k].kind == VEXB_TERM_SPMV) out->term[k].pad[0] = (uint8_t)newslot[out->term[k].pad[0]];
+    for (int k = 0; k < out->n_terms; ++k) if (used[k] && is_product_term(out->term[k].kind)) out->term[k].pad[0] = (uint8_t)newslot[out->term[k].pad[0]];
     for (int k = 0; k < out->n_terms; ++k) if (used[k] && newslot[k] != k) out->term[newslot[k]] = out->term[k];
     for (int k = n; k < out->n_terms; ++k) memset(&out->term[k], 0, sizeof(vexb_term));
     out->n_terms = n;

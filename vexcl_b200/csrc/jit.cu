@@ -9,6 +9,7 @@
 #include "exprhost.hpp"
 #include "jit.hpp"
 #include "spmat.hpp"
+#include "ccsr.hpp"
 #include "peer.cuh"
 #include "fold_text.inc"       // kFoldText: csrc/fold.cuh byte for byte, stringified by vexcl_b200/build.py
 #include <dlfcn.h>
@@ -112,7 +113,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
     bool any_spmv = false;
     for (int comp = 1; comp < ncomp; ++comp)
         for (int k = 0; k < es[comp]->n_terms; ++k)
-            VEXB_CHECK(es[comp]->term[k].kind != VEXB_TERM_SPMV, "sparse products are not fused into multi-expression kernels");
+            VEXB_CHECK(!is_product_term(es[comp]->term[k].kind), "sparse products are not fused into multi-expression kernels");
     for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_SPMV) {
         VEXB_CHECK(ncomp == 1, "sparse products are not fused into multi-expression kernels");
         const vexb_spmat *A = static_cast<const vexb_spmat *>(e.term[k].v.ptr);
@@ -199,6 +200,34 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
         }
         s << "  return sum;\n}\n";
     }
+    // CCSR products used as terminals (VEXB_TERM_CCSR): one row function per terminal, specialised to the value type and
+    // the idx width (pad[1]) only -- never to the matrix, whose handle is not read here -- so one kernel serves every CCSR
+    // matrix of that shape.  The row loop of ccsr_kernel: idx[i], then the unique row's entries through the read-only path
+    // (the table is a few dozen bytes, and interior rows of a warp share one unique row), up to 8 gathers in flight, the
+    // products added in storage order as separate operations (--fmad=false): the bits of vexb_ccsr_spmv(alpha = 1).
+    bool any_ccsr = false;
+    for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_CCSR) {
+        VEXB_CHECK(ncomp == 1, "sparse products are not fused into multi-expression kernels");
+        const int w = e.term[k].pad[1];
+        VEXB_CHECK(w == 1 || w == 2 || w == 4, "term %d: CCSR idx width %d is not 1, 2 or 4", k, w);
+        const char *T = ctype(e.term[k].dtype);
+        const char *IT = w == 1 ? "unsigned char" : w == 2 ? "unsigned short" : "int";
+        if (!any_ccsr) {
+            s << "struct ccsr_desc_j { const void *idx; const int *row; const int *col; const void *val; };\n";
+            any_ccsr = true;
+        }
+        s << "__device__ __forceinline__ " << T << " ccsr_" << k << "(const ccsr_desc_j *__restrict__ m, const " << T
+          << " *__restrict__ x, unsigned long long i) {\n"
+             "  const int u = (int)__ldg((const " << IT << " *)m->idx + i);\n"
+             "  const int *__restrict__ cp = m->col; const " << T << " *__restrict__ vp = (const " << T << " *)m->val;\n"
+             "  const " << T << " *xi = x + i;\n"
+             "  " << T << " sum = 0;\n"
+             "  for (int j = __ldg(m->row + u), e = __ldg(m->row + u + 1); j < e; j += 8) {\n"
+             "    " << T << " xv[8];\n"
+             "#pragma unroll\n    for (int q = 0; q < 8; ++q) xv[q] = j + q < e ? __ldg(xi + __ldg(cp + j + q)) : (" << T << ")0;\n"
+             "#pragma unroll\n    for (int q = 0; q < 8; ++q) if (j + q < e) sum = sum + __ldg(vp + j + q) * xv[q];\n"
+             "  }\n  return sum;\n}\n";
+    }
     const char *LT = ctype(lhs_dtype);
     // One element of the assignment as a function; the kernel below evaluates four of them (a grid stride apart) before it
     // stores any, so a thread has 4 x (number of vector operands) loads in flight instead of one round trip per element.
@@ -222,6 +251,8 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
             else if (tm.kind == VEXB_TERM_SPMV) r << "spmv_" << k << "((const spmv_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
                                                   << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i"
                                                   << (static_cast<const vexb_spmat *>(tm.v.ptr)->fmt == VEXB_FMT_SELL ? ", t)" : ")");
+            else if (tm.kind == VEXB_TERM_CCSR) r << "ccsr_" << k << "((const ccsr_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
+                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i)";
             else if (tm.kind == VEXB_TERM_SCALAR) r << "tt.t[" << k << "].v." << ufield(rt);
             else r << "off + i + (unsigned long long)tt.t[" << k << "].v.i64";
         } else if (op == VEXB_OP_CVT) {
@@ -307,7 +338,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
     }
     s << "}\n";
     }   // components
-    *spmv = any_spmv;
+    *spmv = any_spmv || any_ccsr;
     return VEXB_OK;
 }
 
@@ -584,6 +615,8 @@ static std::string request_signature(const vexb_expr &e, int lhs_dtype, int aop)
             k.push_back((char)e.term[t].pad[0]); k.push_back((char)A->fmt); k.push_back(A->ell_class ? 3 : A->ell_mask ? 2 : A->ell_col16 || A->sell_col16 ? 1 : 0); k.push_back(A->tail_nnz ? 1 : 0);
             const unsigned w = (unsigned)A->ell_width;
             k.push_back((char)(w & 0xff)); k.push_back((char)((w >> 8) & 0xff)); k.push_back((char)((w >> 16) & 0xff)); k.push_back((char)(w >> 24));
+        } else if (e.term[t].kind == VEXB_TERM_CCSR) {   // x's slot and the idx width; never the matrix
+            k.push_back((char)e.term[t].pad[0]); k.push_back((char)e.term[t].pad[1]);
         }
     }
     return k;
@@ -600,8 +633,24 @@ static int pack_terms(const vexb_expr &e, int dev, size_t n, terms_host *tt) {
             VEXB_CHECK(A->dev == dev, "term %d: the matrix lives on device %d, not %d", k, A->dev, dev);
             VEXB_CHECK(A->nrows_stored >= n, "term %d: the strip has %zu rows, the expression %zu elements", k, A->nrows_stored, n);
             tt->t[k].v.ptr = A->d_desc;
+        } else if (e.term[k].kind == VEXB_TERM_CCSR) {
+            void *desc = nullptr;
+            VEXB_TRY(ccsr_term_desc(static_cast<const vexb_ccsr *>(e.term[k].v.ptr), &desc));
+            tt->t[k].v.ptr = desc;
         }
     }
+    return VEXB_OK;
+}
+
+// The CCSR terminals of a request against their handles, before anything is compiled or launched.  lhs: the assignment's
+// target (NULL for reductions); a kernel that writes x[i] while other threads read x[i + col[j]] would race, so an x that
+// is the target is VEXB_ERR_UNSUPPORTED (the front ends evaluate the product into a temporary first).
+static int check_ccsr_terms(const vexb_expr &e, int dev, const void *lhs, size_t n, size_t index_offset) {
+    for (int k = 0; k < e.n_terms; ++k) if (e.term[k].kind == VEXB_TERM_CCSR)
+        VEXB_TRY(ccsr_term_check(static_cast<const vexb_ccsr *>(e.term[k].v.ptr), k, dev, e.term[k].dtype, e.term[k].pad[1], n, index_offset));
+    for (int k = 0; k < e.n_terms; ++k)
+        if (e.term[k].kind == VEXB_TERM_CCSR && lhs && e.term[e.term[k].pad[0]].v.ptr == lhs)
+            VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "term %d: the CCSR product's x is the assignment's target; evaluate the product into a temporary first", k);
     return VEXB_OK;
 }
 
@@ -679,6 +728,7 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     *done = false;
     int sell = -1;
     VEXB_TRY(sell_sweep_term(e, &sell));                              // before the cache: the signature does not tell strips apart
+    VEXB_TRY(check_ccsr_terms(e, dev, lhs, n, index_offset));
     std::shared_ptr<JitEntry> en;
     {
         std::lock_guard<std::mutex> lock(g_jmx);                      // short: map lookup only
@@ -733,7 +783,7 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     unsigned long long nn = n, off = index_offset;
     void *args[] = {&tt, &lhs, &nn, &off};
     bool any_spmv = false;
-    for (int k = 0; k < e.n_terms; ++k) any_spmv = any_spmv || e.term[k].kind == VEXB_TERM_SPMV;
+    for (int k = 0; k < e.n_terms; ++k) any_spmv = any_spmv || is_product_term(e.term[k].kind);
     const size_t per_block = any_spmv ? 256 : 1024;                    // elements per block and loop trip (generate_source: U = 1 / 4)
     size_t blocks = (n + per_block - 1) / per_block;
     const size_t cap = (size_t)sm_count(dev) * 64;
@@ -754,7 +804,7 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
     *done = false;
     if (ncomp < 2 || ncomp > 8) return VEXB_OK;
     for (int c = 0; c < ncomp; ++c)
-        for (int k = 0; k < es[c]->n_terms; ++k) if (es[c]->term[k].kind == VEXB_TERM_SPMV) return VEXB_OK;
+        for (int k = 0; k < es[c]->n_terms; ++k) if (is_product_term(es[c]->term[k].kind)) return VEXB_OK;
     std::string key(1, (char)ncomp);
     for (int c = 0; c < ncomp; ++c) { key += request_signature(*es[c], lhs_dtype, aop); key.push_back('|'); }
     std::shared_ptr<JitEntry> en;
@@ -874,6 +924,7 @@ int jit_reduce(int dev, cudaStream_t st, const vexb_expr &e, int dtype, size_t n
                bool multi, size_t cap, void *d_result, void *d_workspace, const PeerArgs &pa) {
     static std::mutex mx;
     static std::map<std::pair<std::string, int>, void *> fns;
+    VEXB_TRY(check_ccsr_terms(e, dev, nullptr, n, index_offset));
     const int skel = reduce_skeleton(e, dtype, multi);
     std::string key = "reduce:" + request_signature(e, host_result_type(e), VEXB_SET);
     key.push_back('|'); key.push_back((char)dtype); key.push_back((char)skel); key.push_back((char)nops);

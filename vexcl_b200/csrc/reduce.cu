@@ -334,7 +334,7 @@ extern "C" int vexb_reduce_all(int dev, void *stream, const vexb_expr *expr, int
     if (bps < 1) bps = 1; if (bps > kMaxBlocksPerSm) bps = kMaxBlocksPerSm;
     const size_t cap = (size_t)sms * (size_t)bps;
     // user functions and inlined sparse products have no pre-compiled form: one kernel generated for the request (jit.cu)
-    if (expr_has_call(e) || expr_has_spmv(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, 1, &op, false, cap, d_result, d_workspace, pa);
+    if (expr_has_call(e) || expr_has_product(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, 1, &op, false, cap, d_result, d_workspace, pa);
 
     if ((dtype == VEXB_F64 || dtype == VEXB_F32) && !param("eval.force_interp", 0)) {
         ShapeMatch m = match_shape(e, dtype);
@@ -460,7 +460,7 @@ extern "C" int vexb_reduce_multi(int dev, void *stream, const vexb_expr *expr, i
     size_t want = (n + 1023) / 1024;
     const int blocks = (int)(want < cap ? want : cap);
     cudaStream_t st = (cudaStream_t)stream;
-    if (expr_has_call(e) || expr_has_spmv(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, nops, mo.op, true, cap, d_result, d_workspace, pa);
+    if (expr_has_call(e) || expr_has_product(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, nops, mo.op, true, cap, d_result, d_workspace, pa);
     switch (dtype) {
         case VEXB_F64: launch_rmulti<double>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
         case VEXB_F32: launch_rmulti<float>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
