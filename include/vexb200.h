@@ -259,6 +259,29 @@ int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int assign_op,
  * path instead of the interpreter.  Registering the same definition twice returns the same id. */
 int vexb_function_register(const char *name, int ret_dtype, int nargs, const int *arg_dtypes,
                            const char *body, int *id);
+/* The same with dependencies and a preamble (VEX_FUNCTION_D / _SD / _DS, VEX_FUNCTION_V1_WITH_PREAMBLE,
+ * vexcl/function.hpp:70-203); vexb_function_register is this with ndeps = 0 and no preamble.
+ *   deps[0..ndeps) (ndeps <= 64): ids of functions registered before, which `body` calls by their plain names.  A
+ *     program that calls this function holds the closure of the dependency lists, post-order as written (a dependency
+ *     before its dependents), each function of it once and under its plain name `name`; the called function itself
+ *     is emitted as name_<id>, and under its plain name as well when it is also a dependency.  Two distinct functions
+ *     with one plain name in a program's dependencies: VEXB_ERR_INVALID, before NVRTC runs.
+ *   preamble (NULL or ""): file-scope text emitted once per program, before the function's first definition.  A
+ *     program with a preamble is compiled with NVRTC --device-as-default-execution-space, so helpers in it may be
+ *     written without __device__.
+ * The same (name, ret_dtype, arg_dtypes, body, deps, preamble) returns the same id. */
+int vexb_function_register_ex(const char *name, int ret_dtype, int nargs, const int *arg_dtypes, const char *body,
+                              int ndeps, const int *deps, const char *preamble, int *id);
+/* Program headers (vex::push_program_header, backend/common.hpp:120-206): a stack per device ordinal, host state only
+ * (no device is touched).  A push replaces the effective header (the top), a pop restores the previous one; popping an
+ * empty stack is VEXB_ERR_INVALID.  The effective header of `dev` goes at the very top of every program compiled for dev
+ * that carries user text -- vexb_eval, vexb_eval_multi, vexb_reduce_all and vexb_reduce_multi kernels that call a user
+ * function, vexb_stencil_operator_apply and vexb_usr_spmv -- and into those kernels' cache keys; a background
+ * compilation uses the header in effect when it was requested.  _get: the effective header ("" when none), two-call
+ * pattern on *len. */
+int vexb_program_header_push(int dev, const char *text);
+int vexb_program_header_pop(int dev);
+int vexb_program_header_get(int dev, char *buf, size_t *len);
 /* Generated source and NVRTC build log of the kernel vexb_eval would JIT for this request (for inspection
  * and for tests on machines without a GPU: NVRTC needs no device).  Two-call pattern on *len. */
 int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile);
@@ -268,6 +291,13 @@ int vexb_jit_source_multi(int lhs_dtype, int assign_op, int ncomp, const vexb_ex
  * vexb_reduce_all generates when nops == 1 (ops[0]: any vexb_reduce_op), the one vexb_reduce_multi generates when
  * nops > 1 (SUM / SUM_KAHAN / MAX / MIN).  The skeleton follows the tunables in force, as at a launch. */
 int vexb_jit_source_reduce(int dtype, int nops, const int *ops, const vexb_expr *expr, char *buf, size_t *len, int compile);
+/* The three above as device `dev` would compile them now: its program header first when the program calls a user
+ * function.  dev = -1 is the header-less text of the functions above.  No device is touched. */
+int vexb_jit_source_dev(int dev, int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile);
+int vexb_jit_source_multi_dev(int dev, int lhs_dtype, int assign_op, int ncomp, const vexb_expr *const *exprs, char *buf,
+                              size_t *len, int compile);
+int vexb_jit_source_reduce_dev(int dev, int dtype, int nops, const int *ops, const vexb_expr *expr, char *buf, size_t *len,
+                               int compile);
 /* Expressions without a hand-written sweep are served by the pre-compiled interpreter while NVRTC builds a kernel
  * specialised to the expression on a background thread (started at the first use of a new expression shape; tunable
  * "eval.jit": 0 = interpreter only, 1 = compile synchronously, 2 = this, the default).  *pending = 1 while any such

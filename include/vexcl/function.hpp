@@ -6,11 +6,14 @@
  * The result type is the common type of the arguments (as the reference assumes,
  * operations.hpp:1750-1764); integer arguments of floating-only functions are promoted to double.
  *
- * User-defined functions (VEX_FUNCTION and friends, function.hpp:225) carry a C source body; expressions
- * that call one are compiled at first use by the library's NVRTC side path (csrc/jit.cu) and cached.
+ * User-defined functions (VEX_FUNCTION and friends, function.hpp:46-225) carry a C source body, optionally a list of
+ * user functions the body calls by name (VEX_FUNCTION_D / _SD / _DS) or a file-scope preamble
+ * (VEX_FUNCTION_V1_WITH_PREAMBLE); expressions that call one are compiled at first use by the library's NVRTC side
+ * path (csrc/jit.cu) and cached.
  */
 #include <cctype>
 #include <string>
+#include <type_traits>
 #include "operations.hpp"
 
 namespace vex {
@@ -143,7 +146,9 @@ struct call_node : vector_expr_tag {
         }
 };
 
-/// Base of the objects the VEX_FUNCTION macros define.  Impl supplies fn_name(), fn_types(), fn_body().
+/// Base of the objects the VEX_FUNCTION macros define.  Impl supplies fn_name(), fn_types(), fn_deps(), fn_preamble()
+/// and fn_body().  Dependencies are registered first (their ids come from their own id()), so a function's id is always
+/// larger than those of the functions its body calls.
 template <class Impl, class Ret>
 struct user_function {
     typedef Ret result_type;
@@ -152,9 +157,13 @@ struct user_function {
         static const int fid = [] {
             std::string prologue;
             Impl::fn_types(types, prologue);
+            std::vector<int> deps;
+            Impl::fn_deps(deps);
+            const std::string preamble = Impl::fn_preamble();
             int k = -1;
-            VEXB_CHECKED(vexb_function_register(Impl::fn_name(), dtype_of<typename detail::promoted<Ret>::type>::value,
-                                                static_cast<int>(types.size()), types.data(), (prologue + Impl::fn_body()).c_str(), &k));
+            VEXB_CHECKED(vexb_function_register_ex(Impl::fn_name(), dtype_of<typename detail::promoted<Ret>::type>::value,
+                                                   static_cast<int>(types.size()), types.data(), (prologue + Impl::fn_body()).c_str(),
+                                                   static_cast<int>(deps.size()), deps.data(), preamble.c_str(), &k));
             return k;
         }();
         if (types_out) *types_out = types;
@@ -171,25 +180,59 @@ struct user_function {
 
 } // namespace vex
 
+/// Converts unquoted text into a string literal (function.hpp:46).
+#define VEX_STRINGIZE_SOURCE(...) #__VA_ARGS__
+
+// The dependency sequence (f)(g)(h) of VEX_FUNCTION_D / _SD as statements `deps.push_back(<id of f>);`, one per element:
+// the two macros call each other through the sequence and the last one left is pasted into an empty *_END.
+#define VEXCL_FUNCTION_DEP_0(dep) deps.push_back(std::decay<decltype(dep)>::type::id()); VEXCL_FUNCTION_DEP_1
+#define VEXCL_FUNCTION_DEP_1(dep) deps.push_back(std::decay<decltype(dep)>::type::id()); VEXCL_FUNCTION_DEP_0
+#define VEXCL_FUNCTION_DEP_0_END
+#define VEXCL_FUNCTION_DEP_1_END
+#define VEXCL_FUNCTION_CAT(a, b) VEXCL_FUNCTION_CAT_I(a, b)
+#define VEXCL_FUNCTION_CAT_I(a, b) a##b
+#define VEXCL_FUNCTION_DEPS(seq) VEXCL_FUNCTION_CAT(VEXCL_FUNCTION_DEP_0 seq, _END)
+
+/// The object `fname` of type vex_function_fname, registered under the plain name "fname" (the name dependents call).
+#define VEXCL_FUNCTION_SINK(rettype, fname, fargs, dependencies, preamble_str, body_str) \
+    struct vex_function_##fname : vex::user_function<vex_function_##fname, rettype> { \
+        vex_function_##fname() {} \
+        static const char* fn_name() { return #fname; } \
+        static void fn_types(std::vector<int> &t, std::string &prologue) { vex::detail::parse_arguments(#fargs, t, prologue); } \
+        static void fn_deps(std::vector<int> &deps) { (void)deps; VEXCL_FUNCTION_DEPS(dependencies) } \
+        static std::string fn_preamble() { return preamble_str; } \
+        static std::string fn_body() { return body_str; } \
+    } const fname
+
+/// VEX_FUNCTION_SD(return_type, name, (type1, arg1)..., (dep1)(dep2)..., body_str)   -- function.hpp:194-203
+/// A function whose body calls the user functions dep1, dep2, ... by name; they are compiled into every program that
+/// calls it.
+#define VEX_FUNCTION_SD(rettype, fname, fargs, dependencies, body_str) \
+    VEXCL_FUNCTION_SINK(rettype, fname, fargs, dependencies, "", body_str)
+#define VEX_FUNCTION_DS VEX_FUNCTION_SD
+/// Same with the body as unquoted source.
+#define VEX_FUNCTION_D(rettype, fname, fargs, dependencies, ...) \
+    VEX_FUNCTION_SD(rettype, fname, fargs, dependencies, #__VA_ARGS__)
 /// VEX_FUNCTION(return_type, name, (type1, arg1)(type2, arg2)..., body)      -- function.hpp:225
 #define VEX_FUNCTION(rettype, fname, fargs, ...) VEX_FUNCTION_S(rettype, fname, fargs, #__VA_ARGS__)
 /// Same with the body given as a string.
-#define VEX_FUNCTION_S(rettype, fname, fargs, body_str) \
-    VEX_FUNCTION_SD(rettype, vex_function_##fname, fargs, body_str) const fname
-/// Define the function *type* only (instantiate it yourself).
-#define VEX_FUNCTION_D(rettype, ftype, fargs, ...) VEX_FUNCTION_SD(rettype, ftype, fargs, #__VA_ARGS__)
-#define VEX_FUNCTION_SD(rettype, ftype, fargs, body_str) \
-    struct ftype : vex::user_function<ftype, rettype> { \
-        static const char* fn_name() { return #ftype; } \
-        static void fn_types(std::vector<int> &t, std::string &prologue) { vex::detail::parse_arguments(#fargs, t, prologue); } \
-        static std::string fn_body() { return body_str; } \
-    }
-/// Older form: VEX_FUNCTION_V1(name, double(double, double), "return prm1 + prm2;")
-#define VEX_FUNCTION_V1(fname, signature, body_str) \
+#define VEX_FUNCTION_S(rettype, fname, fargs, body_str) VEX_FUNCTION_SD(rettype, fname, fargs, , body_str)
+
+/// Older form, the type only: VEX_FUNCTION_V1_TYPE(name, double(double, double), preamble_str, "return prm1 + prm2;")
+/// defines vex_function_name (function.hpp:70-118).  The preamble is file-scope text (helpers, macros) before the body.
+#define VEX_FUNCTION_V1_TYPE(fname, signature, preamble_str, body_str) \
     struct vex_function_##fname : vex::user_function<vex_function_##fname, vex::detail::signature_types<signature>::result> { \
+        vex_function_##fname() {} \
         static const char* fn_name() { return #fname; } \
         static void fn_types(std::vector<int> &t, std::string&) { t = vex::detail::signature_types<signature>::args(); } \
+        static void fn_deps(std::vector<int>&) {} \
+        static std::string fn_preamble() { return preamble_str; } \
         static std::string fn_body() { return body_str; } \
-    } const fname
+    }
+/// VEX_FUNCTION_V1(name, double(double, double), "return prm1 + prm2;")
+#define VEX_FUNCTION_V1(fname, signature, body_str) VEX_FUNCTION_V1_TYPE(fname, signature, "", body_str) const fname
+/// VEX_FUNCTION_V1_WITH_PREAMBLE(name, double(double), "double sq(double x) { return x * x; }\n", "return sq(prm1);")
+#define VEX_FUNCTION_V1_WITH_PREAMBLE(fname, signature, preamble_str, body_str) \
+    VEX_FUNCTION_V1_TYPE(fname, signature, preamble_str, body_str) const fname
 
 #endif

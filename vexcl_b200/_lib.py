@@ -141,6 +141,13 @@ def lib():
         "vexb_jit_source": ([i, i, P(Expr), C.c_char_p, P(sz), i], i),
         "vexb_jit_source_multi": ([i, i, i, P(P(Expr)), C.c_char_p, P(sz), i], i),
         "vexb_jit_source_reduce": ([i, i, P(i), P(Expr), C.c_char_p, P(sz), i], i),
+        "vexb_function_register_ex": ([C.c_char_p, i, i, P(i), C.c_char_p, i, P(i), C.c_char_p, P(i)], i),
+        "vexb_program_header_push": ([i, C.c_char_p], i),
+        "vexb_program_header_pop": ([i], i),
+        "vexb_program_header_get": ([i, C.c_char_p, P(sz)], i),
+        "vexb_jit_source_dev": ([i, i, i, P(Expr), C.c_char_p, P(sz), i], i),
+        "vexb_jit_source_multi_dev": ([i, i, i, i, P(P(Expr)), C.c_char_p, P(sz), i], i),
+        "vexb_jit_source_reduce_dev": ([i, i, i, P(i), P(Expr), C.c_char_p, P(sz), i], i),
         "vexb_reduce_workspace_bytes": ([i, P(sz)], i),
         "vexb_reduce": ([i, vp, P(Expr), i, sz, sz, i, vp, vp], i),
         "vexb_reduce_identity": ([i, vp, i, i, vp], i),

@@ -301,22 +301,58 @@ class Call(Node):
 class UserFunction:
     """VEX_FUNCTION(ret, name, (type, arg)..., body) (vexcl/function.hpp:225): a device function given as C source.
     `args` is a list of (numpy dtype, name); inside `body` the arguments are available under their names (and, as in
-    the reference's older form, as prm1, prm2, ...).  Expressions that call it run on the NVRTC side path."""
+    the reference's older form, as prm1, prm2, ...).  Expressions that call it run on the NVRTC side path.
+    deps: UserFunctions the body calls by their names (VEX_FUNCTION_D); every program that calls this one holds them.
+    preamble: file-scope text (helpers, macros) before the definition (VEX_FUNCTION_V1_WITH_PREAMBLE); helpers in it
+    need no __device__."""
 
-    def __init__(self, ret, name: str, args, body: str):
+    def __init__(self, ret, name: str, args, body: str, deps=(), preamble: str = ""):
         self.ret = _vdt(ret)
         self.arg_types = [_vdt(t) for t, _ in args]
         ctypes_names = {L.F64: "double", L.F32: "float", L.I32: "int", L.U32: "unsigned int", L.I64: "long long", L.U64: "unsigned long long"}
         prologue = "".join(f"const {ctypes_names[t]} {nm} = prm{k + 1}; " for k, (t, (_, nm)) in enumerate(zip(self.arg_types, args)))
         fid = C.c_int(-1)
         at = (C.c_int * max(len(args), 1))(*self.arg_types)
-        L.check(L.lib().vexb_function_register(name.encode(), self.ret, len(args), at, (prologue + body).encode(), C.byref(fid)))
+        dep_ids = [d.id if isinstance(d, UserFunction) else int(d) for d in deps]
+        if dep_ids or preamble:
+            da = (C.c_int * max(len(dep_ids), 1))(*dep_ids)
+            L.check(L.lib().vexb_function_register_ex(name.encode(), self.ret, len(args), at, (prologue + body).encode(),
+                                                      len(dep_ids), da, preamble.encode(), C.byref(fid)))
+        else:
+            L.check(L.lib().vexb_function_register(name.encode(), self.ret, len(args), at, (prologue + body).encode(), C.byref(fid)))
         self.id, self.name = fid.value, name
 
     def __call__(self, *args):
         if len(args) != len(self.arg_types):
             raise TypeError(f"{self.name} takes {len(self.arg_types)} arguments")
         return Call(self, args)
+
+
+def _header_devices(ctx: Context):
+    return sorted(set(ctx.devs[k] for k in ctx.local))
+
+
+def push_program_header(ctx: Context, text: str):
+    """vex::push_program_header(ctx, text) (backend/common.hpp:120-206): `text` goes at the very top of every kernel
+    compiled from user text (expressions that call a UserFunction, stencil operators, user value types) on each device
+    of ctx, once per distinct device.  It replaces the previous header until pop_program_header(ctx)."""
+    for d in _header_devices(ctx):
+        L.check(L.lib().vexb_program_header_push(d, text.encode()))
+
+
+def pop_program_header(ctx: Context):
+    """Restores the program header each device of ctx had before the last push."""
+    for d in _header_devices(ctx):
+        L.check(L.lib().vexb_program_header_pop(d))
+
+
+def program_header(dev: int) -> str:
+    """The effective program header of device `dev` ("" when none was pushed)."""
+    n = C.c_size_t(0)
+    L.check(L.lib().vexb_program_header_get(dev, None, C.byref(n)))
+    buf = C.create_string_buffer(n.value)
+    L.check(L.lib().vexb_program_header_get(dev, buf, C.byref(n)))
+    return buf.value.decode()
 
 
 def _mkfunc(op):

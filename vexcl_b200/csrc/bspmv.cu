@@ -469,9 +469,11 @@ static std::string usr_source(const vexb_usr_ops &o, size_t val_bytes) {
 static std::mutex g_usr_mx;
 static std::map<std::pair<std::string, int>, void *> g_usr_fns;
 
+// The device's program header goes first in the source (the snippets may use what it declares) and into the key.
 static int usr_kernel(int dev, const vexb_usr_ops &o, size_t val_bytes, void **fn) {
+    const std::string header = program_header(dev);
     std::string key;
-    for (const char *part : {o.val_type, o.rhs_type, o.decl, o.product, o.append}) {
+    for (const char *part : {o.val_type, o.rhs_type, o.decl, o.product, o.append, header.c_str()}) {
         key += std::to_string(strlen(part)); key += ':'; key += part;
     }
     key += std::to_string(o.rhs_bytes) + ":" + std::to_string(val_bytes);
@@ -481,7 +483,7 @@ static int usr_kernel(int dev, const vexb_usr_ops &o, size_t val_bytes, void **f
         auto it = g_usr_fns.find(k);
         if (it != g_usr_fns.end()) { *fn = it->second; return VEXB_OK; }
     }
-    VEXB_TRY(jit_build(dev, usr_source(o, val_bytes), "vexb_usr_kernel", fn));
+    VEXB_TRY(jit_build(dev, with_program_header(header, usr_source(o, val_bytes)), "vexb_usr_kernel", fn));
     std::lock_guard<std::mutex> lock(g_usr_mx);
     g_usr_fns[k] = *fn;
     return VEXB_OK;

@@ -18,15 +18,37 @@
 #include <mutex>
 #include <condition_variable>
 #include <memory>
+#include <functional>
 #include <thread>
 #include <sstream>
 #include <vector>
 
 namespace vexb {
 
-struct UserFunc { std::string name; int ret; std::vector<int> args; std::string body; };
+// deps: ids of functions registered earlier, which the body calls by their plain names; preamble: file-scope text
+// (helpers, macros) that the body may use (VEX_FUNCTION_D / _SD, VEX_FUNCTION_V1_WITH_PREAMBLE, vexcl/function.hpp).
+struct UserFunc { std::string name; int ret; std::vector<int> args; std::string body; std::vector<int> deps; std::string preamble; };
 static std::mutex g_fmx;
 static std::vector<UserFunc> g_funcs;
+constexpr int kMaxDeps = 64;                        // entries of one dependency list
+
+// Program headers (vex::push_program_header, backend/common.hpp): a stack per device ordinal.  A push replaces the
+// effective header (the top), a pop restores the one before.  It goes at the very top of every program compiled for that
+// device that carries user text, and is part of those kernels' cache keys.
+constexpr int kMaxHeaderDevices = 1024;
+static std::mutex g_hdr_mx;
+static std::map<int, std::vector<std::string>> g_headers;
+
+std::string program_header(int dev) {
+    std::lock_guard<std::mutex> l(g_hdr_mx);
+    auto it = g_headers.find(dev);
+    return it == g_headers.end() || it->second.empty() ? std::string() : it->second.back();
+}
+
+std::string with_program_header(const std::string &header, const std::string &src) {
+    if (header.empty()) return src;
+    return header + (header.back() == '\n' ? "" : "\n") + src;
+}
 
 int function_arity(int id) { std::lock_guard<std::mutex> l(g_fmx); return (id >= 0 && id < (int)g_funcs.size()) ? (int)g_funcs[id].args.size() : -1; }
 int function_arg_dtype(int id, int k) { std::lock_guard<std::mutex> l(g_fmx); return g_funcs[id].args[k]; }
@@ -63,6 +85,79 @@ static const char *math_name(int op) {
     return "";
 }
 
+// The user functions of a program.  A function the expression calls is emitted as name_<id>, after the closure of its
+// dependency lists: post-order over the lists as written, every function of it once and under its plain name, the name
+// its dependents' bodies use (so a called function that is also a dependency appears under both names).  A function's
+// preamble goes once, before its first definition.  Two distinct functions with one plain name are refused here, before
+// NVRTC sees the program.  Without dependencies and preambles the text is that of the called functions alone.
+static int emit_user_functions(const vexb_expr *const *es, int ncomp, std::ostream &s) {
+    std::lock_guard<std::mutex> l(g_fmx);
+    const size_t nf = g_funcs.size();
+    std::vector<bool> called(nf, false), plain(nf, false), pre(nf, false);
+    std::map<std::string, int> plain_ids;
+    auto define = [&](int id, bool as_plain) {
+        const UserFunc &f = g_funcs[id];
+        if (!f.preamble.empty() && !pre[id]) {
+            pre[id] = true;
+            s << f.preamble << (f.preamble.back() == '\n' ? "" : "\n");
+        }
+        s << "__device__ __forceinline__ " << ctype(f.ret) << " " << f.name;
+        if (!as_plain) s << "_" << id;
+        s << "(";
+        for (size_t k = 0; k < f.args.size(); ++k) s << (k ? ", " : "") << ctype(f.args[k]) << " prm" << (k + 1);
+        s << ") {\n" << f.body << "\n}\n";
+    };
+    std::function<int(int)> dependency = [&](int id) -> int {
+        if (plain[id]) return VEXB_OK;
+        plain[id] = true;
+        auto ins = plain_ids.emplace(g_funcs[id].name, id);
+        if (!ins.second) VEXB_FAIL(VEXB_ERR_INVALID, "user functions %d and %d are both named '%s' among the dependencies of one program",
+                                   ins.first->second, id, g_funcs[id].name.c_str());
+        for (int d : g_funcs[id].deps) VEXB_TRY(dependency(d));
+        define(id, true);
+        return VEXB_OK;
+    };
+    for (int comp = 0; comp < ncomp; ++comp)
+        for (int pc = 0; pc < es[comp]->n_code; ++pc) if (es[comp]->code[pc].op == VEXB_OP_CALL && !called[es[comp]->code[pc].arg]) {
+            const int id = es[comp]->code[pc].arg; called[id] = true;
+            for (int d : g_funcs[id].deps) VEXB_TRY(dependency(d));
+            define(id, false);
+        }
+    return VEXB_OK;
+}
+
+// Whether a program needs NVRTC's --device-as-default-execution-space: some function it calls, or one of their
+// dependencies, has a preamble, whose helpers are written without __device__ (the reference's own example does so).
+static bool program_has_preamble(const vexb_expr *const *es, int ncomp) {
+    std::lock_guard<std::mutex> l(g_fmx);
+    std::vector<bool> seen(g_funcs.size(), false);
+    std::function<bool(int)> walk = [&](int id) {
+        if (seen[id]) return false;
+        seen[id] = true;
+        if (!g_funcs[id].preamble.empty()) return true;
+        for (int d : g_funcs[id].deps) if (walk(d)) return true;
+        return false;
+    };
+    for (int comp = 0; comp < ncomp; ++comp)
+        for (int pc = 0; pc < es[comp]->n_code; ++pc)
+            if (es[comp]->code[pc].op == VEXB_OP_CALL && walk(es[comp]->code[pc].arg)) return true;
+    return false;
+}
+
+// The header of device `dev` for a program, or "" when the program carries no user text (no call) or dev < 0 (the
+// source printers without a device).
+static std::string header_for(int dev, const vexb_expr *const *es, int ncomp) {
+    if (dev < 0) return std::string();
+    for (int comp = 0; comp < ncomp; ++comp) if (expr_has_call(*es[comp])) return program_header(dev);
+    return std::string();
+}
+
+// A cache key extended by the header it was compiled under; keys of programs without a header stay as they were.
+static std::string key_with_header(std::string key, const std::string &header) {
+    if (!header.empty()) { key.push_back('\0'); key += "header:"; key += header; }
+    return key;
+}
+
 // Print a normalised program as CUDA C.  One `const T rK = ...;` per instruction keeps the text linear in
 // the program length; the semantics of every operator mirror csrc/expr_eval.cuh.
 // ncomp > 1: the components of a multi-expression assignment (vex::tie(a, b) = std::tie(e0, e1), multivector
@@ -94,18 +189,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
          "struct term_j { unsigned char kind, dtype, pad[6]; union { const void *ptr; double f64; float f32; int i32;"
          " unsigned int u32; long long i64; unsigned long long u64; } v; };\n"
          "struct terms_j { term_j t[" << VEXB_MAX_TERMS << "]; };\n";
-    {   // user functions used by this program
-        std::lock_guard<std::mutex> l(g_fmx);
-        std::vector<bool> seen(g_funcs.size(), false);
-        for (int comp = 0; comp < ncomp; ++comp)
-        for (int pc = 0; pc < es[comp]->n_code; ++pc) if (es[comp]->code[pc].op == VEXB_OP_CALL && !seen[es[comp]->code[pc].arg]) {
-            const int id = es[comp]->code[pc].arg; seen[id] = true;
-            const UserFunc &f = g_funcs[id];
-            s << "__device__ __forceinline__ " << ctype(f.ret) << " " << f.name << "_" << id << "(";
-            for (size_t k = 0; k < f.args.size(); ++k) s << (k ? ", " : "") << ctype(f.args[k]) << " prm" << (k + 1);
-            s << ") {\n" << f.body << "\n}\n";
-        }
-    }
+    VEXB_TRY(emit_user_functions(es, ncomp, s));
     // sparse products used as terminals (VEXB_TERM_SPMV): one row function per terminal, specialised to the strip's format
     // -- hybrid ELL with the width as a literal (fully unrolled: all column/value loads, then all gathers of x, in
     // flight at once, like hell_kernel), 32-bit columns, 16-bit offsets, slot masks or row classes, with or without a CSR tail; or plain CSR, one thread per
@@ -569,15 +653,16 @@ static std::mutex g_nvrtc_mx;
 static std::atomic<bool> g_bg_cancel{false};       // set while the process is leaving: queued compilations give up (see below)
 constexpr int VEXB_ERR_CANCELLED = -100;           // internal only, never returned through the ABI
 
-static int compile_cubin(const std::string &src, std::vector<char> *cubin, std::string *log) {
+// device_default: --device-as-default-execution-space, for programs with a preamble (program_has_preamble) only.
+static int compile_cubin(const std::string &src, std::vector<char> *cubin, std::string *log, bool device_default = false) {
     VEXB_TRY(load_nvrtc());
     std::lock_guard<std::mutex> nvrtc_lock(g_nvrtc_mx);
     if (g_bg_cancel.load()) return VEXB_ERR_CANCELLED;                 // queued behind another compilation while the process exits
     nvrtcProgram prog = nullptr;
     nvrtcResult r = g_jit.nvrtcCreateProgram(&prog, src.c_str(), "vexb_jit.cu", 0, nullptr, nullptr);
     if (r != 0) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "nvrtcCreateProgram: %s", g_jit.nvrtcGetErrorString(r));
-    const char *opts[] = {"--gpu-architecture=sm_90a", "--fmad=false", "--std=c++17", "-lineinfo"};
-    r = g_jit.nvrtcCompileProgram(prog, 4, opts);
+    const char *opts[] = {"--gpu-architecture=sm_90a", "--fmad=false", "--std=c++17", "-lineinfo", "--device-as-default-execution-space"};
+    r = g_jit.nvrtcCompileProgram(prog, device_default ? 5 : 4, opts);
     size_t ls = 0;
     g_jit.nvrtcGetProgramLogSize(prog, &ls);
     std::string lg(ls ? ls : 1, '\0');
@@ -689,13 +774,14 @@ static thread_local BackgroundJoinGuard tl_bg_guard;
 
 // NVRTC front to back for one entry; runs WITHOUT the global lock (hundreds of milliseconds), on the caller's thread
 // (mode 1) or on a background thread (mode 2).
-static void compile_entry(std::shared_ptr<JitEntry> en, std::vector<vexb_expr> es, int lhs_dtype, int aop) {
+// header: the device's program header when the request was made (header_for), "" for none.
+static void compile_entry(std::shared_ptr<JitEntry> en, std::vector<vexb_expr> es, int lhs_dtype, int aop, std::string header) {
     std::string src, err;
     std::vector<char> cubin;
     std::vector<const vexb_expr *> ps;
     for (const vexb_expr &x : es) ps.push_back(&x);
     int st = generate_source_n(ps.data(), (int)ps.size(), lhs_dtype, aop, &src);
-    if (st == VEXB_OK) st = compile_cubin(src, &cubin, nullptr);
+    if (st == VEXB_OK) st = compile_cubin(with_program_header(header, src), &cubin, nullptr, program_has_preamble(ps.data(), (int)ps.size()));
     if (st == VEXB_ERR_CANCELLED) {                                     // the process is leaving: back to "never tried"
         std::lock_guard<std::mutex> lock(en->mx);
         en->state = 0;
@@ -709,11 +795,11 @@ static void compile_entry(std::shared_ptr<JitEntry> en, std::vector<vexb_expr> e
     en->cv.notify_all();
 }
 
-static void spawn_background(std::shared_ptr<JitEntry> en, const std::vector<vexb_expr> &e, int lhs_dtype, int aop) {
+static void spawn_background(std::shared_ptr<JitEntry> en, const std::vector<vexb_expr> &e, int lhs_dtype, int aop, const std::string &header) {
     std::lock_guard<std::mutex> bl(g_bg_mx);
     static bool registered = false;
     if (!registered) { registered = true; atexit(join_background_compilations); }
-    g_bg_threads.emplace_back(compile_entry, en, e, lhs_dtype, aop);
+    g_bg_threads.emplace_back(compile_entry, en, e, lhs_dtype, aop, header);
     tl_bg_guard.armed = true;
 }
 
@@ -729,10 +815,12 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     int sell = -1;
     VEXB_TRY(sell_sweep_term(e, &sell));                              // before the cache: the signature does not tell strips apart
     VEXB_TRY(check_ccsr_terms(e, dev, lhs, n, index_offset));
+    const vexb_expr *pe = &e;
+    const std::string header = header_for(dev, &pe, 1);
     std::shared_ptr<JitEntry> en;
     {
         std::lock_guard<std::mutex> lock(g_jmx);                      // short: map lookup only
-        auto &slot = g_entries[request_signature(e, lhs_dtype, aop)];
+        auto &slot = g_entries[key_with_header(request_signature(e, lhs_dtype, aop), header)];
         if (!slot) slot = std::make_shared<JitEntry>();
         en = slot;
     }
@@ -748,11 +836,11 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
             else {
                 en->state = 1;
                 if (mode == 2 && !param("eval.jit_sync", 0)) {
-                    spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop);
+                    spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop, header);
                     return VEXB_OK;                                    // the interpreter serves meanwhile
                 }
                 lock.unlock();
-                compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop);
+                compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop, header);
                 lock.lock();
             }
         }
@@ -807,10 +895,11 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
         for (int k = 0; k < es[c]->n_terms; ++k) if (is_product_term(es[c]->term[k].kind)) return VEXB_OK;
     std::string key(1, (char)ncomp);
     for (int c = 0; c < ncomp; ++c) { key += request_signature(*es[c], lhs_dtype, aop); key.push_back('|'); }
+    const std::string header = header_for(dev, es, ncomp);
     std::shared_ptr<JitEntry> en;
     {
         std::lock_guard<std::mutex> lock(g_jmx);
-        auto &slot = g_entries["multi:" + key];
+        auto &slot = g_entries[key_with_header("multi:" + key, header)];
         if (!slot) slot = std::make_shared<JitEntry>();
         en = slot;
     }
@@ -826,9 +915,9 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
                 en->state = 1;
                 std::vector<vexb_expr> copy;
                 for (int c = 0; c < ncomp; ++c) copy.push_back(*es[c]);
-                if (mode == 2 && !param("eval.jit_sync", 0)) { spawn_background(en, copy, lhs_dtype, aop); return VEXB_OK; }
+                if (mode == 2 && !param("eval.jit_sync", 0)) { spawn_background(en, copy, lhs_dtype, aop, header); return VEXB_OK; }
                 lock.unlock();
-                compile_entry(en, copy, lhs_dtype, aop);
+                compile_entry(en, copy, lhs_dtype, aop, header);
                 lock.lock();
             }
         }
@@ -878,9 +967,9 @@ int jit_pending() {
 }
 
 // ---- helpers for other run-time specialised kernels (jit.hpp) ---------------------------------------------------------
-int jit_compile_only(const std::string &src, size_t *cubin_bytes, std::string *log) {
+int jit_compile_only(const std::string &src, size_t *cubin_bytes, std::string *log, bool device_default) {
     std::vector<char> cubin;
-    VEXB_TRY(compile_cubin(src, &cubin, log));
+    VEXB_TRY(compile_cubin(src, &cubin, log, device_default));
     if (cubin_bytes) *cubin_bytes = cubin.size();
     return VEXB_OK;
 }
@@ -889,14 +978,14 @@ int jit_compile_only(const std::string &src, size_t *cubin_bytes, std::string *l
 static std::map<std::pair<std::string, int>, CUfunction> g_built;
 static std::mutex g_bmx;
 
-int jit_build(int dev, const std::string &src, const char *name, void **fn) {
-    const std::pair<std::string, int> key(src + "\n//" + name, dev);
+int jit_build(int dev, const std::string &src, const char *name, void **fn, bool device_default) {
+    const std::pair<std::string, int> key(src + "\n//" + name + (device_default ? "\n//device-as-default-execution-space" : ""), dev);
     std::lock_guard<std::mutex> lock(g_bmx);                          // builds are rare and serialised; launches do not come here
     auto it = g_built.find(key);
     if (it != g_built.end()) { *fn = it->second; return VEXB_OK; }
     VEXB_TRY(load_driver());
     std::vector<char> cubin;
-    VEXB_TRY(compile_cubin(src, &cubin, nullptr));
+    VEXB_TRY(compile_cubin(src, &cubin, nullptr, device_default));
     VEXB_CUDA(cudaFree(0));                                           // make sure the primary context is current
     CUmodule mod = nullptr;
     CUfunction f = nullptr;
@@ -926,9 +1015,12 @@ int jit_reduce(int dev, cudaStream_t st, const vexb_expr &e, int dtype, size_t n
     static std::map<std::pair<std::string, int>, void *> fns;
     VEXB_TRY(check_ccsr_terms(e, dev, nullptr, n, index_offset));
     const int skel = reduce_skeleton(e, dtype, multi);
+    const vexb_expr *pe = &e;
+    const std::string header = header_for(dev, &pe, 1);
     std::string key = "reduce:" + request_signature(e, host_result_type(e), VEXB_SET);
     key.push_back('|'); key.push_back((char)dtype); key.push_back((char)skel); key.push_back((char)nops);
     for (int k = 0; k < nops; ++k) key.push_back((char)ops[k]);
+    key = key_with_header(key, header);
     void *fn = nullptr;
     {
         std::lock_guard<std::mutex> lock(mx);
@@ -938,7 +1030,7 @@ int jit_reduce(int dev, cudaStream_t st, const vexb_expr &e, int dtype, size_t n
     if (!fn) {
         std::string src;
         VEXB_TRY(generate_reduce_source(e, dtype, nops, ops, skel, &src));
-        VEXB_TRY(jit_build(dev, src, "vexb_reduce_kernel", &fn));
+        VEXB_TRY(jit_build(dev, with_program_header(header, src), "vexb_reduce_kernel", &fn, program_has_preamble(&pe, 1)));
         std::lock_guard<std::mutex> lock(mx);
         fns[std::make_pair(key, dev)] = fn;
     }
@@ -964,7 +1056,13 @@ using namespace vexb;
 
 extern "C" int vexb_function_register(const char *name, int ret_dtype, int nargs, const int *arg_dtypes,
                                       const char *body, int *id) {
+    return vexb_function_register_ex(name, ret_dtype, nargs, arg_dtypes, body, 0, nullptr, nullptr, id);
+}
+
+extern "C" int vexb_function_register_ex(const char *name, int ret_dtype, int nargs, const int *arg_dtypes, const char *body,
+                                         int ndeps, const int *deps, const char *preamble, int *id) {
     VEXB_CHECK(name && body && id, "NULL argument");
+    VEXB_CHECK(ndeps >= 0 && ndeps <= kMaxDeps && (ndeps == 0 || deps), "a user function lists 0..%d dependencies", kMaxDeps);
     VEXB_CHECK(ret_dtype >= VEXB_F64 && ret_dtype <= VEXB_U64, "bad return type %d", ret_dtype);
     VEXB_CHECK(nargs >= 0 && nargs <= 8 && (nargs == 0 || arg_dtypes), "a user function takes 0..8 arguments");
     VEXB_CHECK(*name && (isalpha((unsigned char)*name) || *name == '_'), "'%s' is not an identifier", name);
@@ -974,9 +1072,19 @@ extern "C" int vexb_function_register(const char *name, int ret_dtype, int nargs
         VEXB_CHECK(arg_dtypes[k] >= VEXB_F64 && arg_dtypes[k] <= VEXB_U64, "bad type of argument %d", k);
         f.args.push_back(arg_dtypes[k]);
     }
+    if (preamble) f.preamble = preamble;
     std::lock_guard<std::mutex> l(g_fmx);
-    for (size_t k = 0; k < g_funcs.size(); ++k)
-        if (g_funcs[k].name == f.name && g_funcs[k].ret == f.ret && g_funcs[k].args == f.args && g_funcs[k].body == f.body) { *id = (int)k; return VEXB_OK; }
+    for (int k = 0; k < ndeps; ++k) {
+        VEXB_CHECK(deps[k] >= 0 && (size_t)deps[k] < g_funcs.size(), "dependency %d: %d is not a registered function", k, deps[k]);
+        f.deps.push_back(deps[k]);
+    }
+    for (size_t k = 0; k < g_funcs.size(); ++k) {
+        const UserFunc &o = g_funcs[k];
+        if (o.name == f.name && o.ret == f.ret && o.args == f.args && o.body == f.body && o.deps == f.deps && o.preamble == f.preamble) {
+            *id = (int)k;
+            return VEXB_OK;
+        }
+    }
     VEXB_CHECK(g_funcs.size() < 65535, "too many user functions");
     g_funcs.push_back(f);
     *id = (int)g_funcs.size() - 1;
@@ -1004,9 +1112,9 @@ extern "C" int vexb_jit_precompile(int lhs_dtype, int assign_op, const vexb_expr
     std::unique_lock<std::mutex> lock(en->mx);
     if (en->state == 0) {
         en->state = 1;
-        if (background) { spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op); return VEXB_OK; }
+        if (background) { spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op, std::string()); return VEXB_OK; }
         lock.unlock();
-        compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op);
+        compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op, std::string());
         lock.lock();
     }
     if (!background && en->state == 1) en->cv.wait(lock, [&] { return en->state != 1; });
@@ -1020,9 +1128,50 @@ extern "C" int vexb_jit_pending(int *pending) {
     return VEXB_OK;
 }
 
+extern "C" int vexb_program_header_push(int dev, const char *text) {
+    VEXB_CHECK(dev >= 0 && dev < kMaxHeaderDevices, "bad device ordinal %d", dev);
+    VEXB_CHECK(text, "text is NULL");
+    std::lock_guard<std::mutex> l(g_hdr_mx);
+    g_headers[dev].push_back(text);
+    return VEXB_OK;
+}
+
+extern "C" int vexb_program_header_pop(int dev) {
+    VEXB_CHECK(dev >= 0 && dev < kMaxHeaderDevices, "bad device ordinal %d", dev);
+    std::lock_guard<std::mutex> l(g_hdr_mx);
+    auto it = g_headers.find(dev);
+    VEXB_CHECK(it != g_headers.end() && !it->second.empty(), "no program header was pushed on device %d", dev);
+    it->second.pop_back();
+    return VEXB_OK;
+}
+
+extern "C" int vexb_program_header_get(int dev, char *buf, size_t *len) {
+    VEXB_CHECK(len, "len is NULL");
+    VEXB_CHECK(dev >= 0 && dev < kMaxHeaderDevices, "bad device ordinal %d", dev);
+    const std::string h = program_header(dev);
+    if (buf) {
+        VEXB_CHECK(*len > h.size(), "buffer too small (%zu <= %zu)", *len, h.size());
+        memcpy(buf, h.c_str(), h.size() + 1);
+    }
+    *len = h.size() + 1;
+    return VEXB_OK;
+}
+
 // The kernel vexb_eval_multi would generate for these components, as text (and, with compile != 0, compiled by NVRTC for
 // sm_90a without touching a device): lets a CPU-only box check that multi-expression kernels build.
 extern "C" int vexb_jit_source_multi(int lhs_dtype, int assign_op, int ncomp, const vexb_expr *const *exprs, char *buf, size_t *len, int compile) {
+    return vexb_jit_source_multi_dev(-1, lhs_dtype, assign_op, ncomp, exprs, buf, len, compile);
+}
+
+// The printers below with dev >= 0 print what device dev would compile, its program header included; dev = -1: no header.
+static int check_print_dev(int dev) {
+    VEXB_CHECK(dev >= -1 && dev < kMaxHeaderDevices, "bad device ordinal %d", dev);
+    return VEXB_OK;
+}
+
+extern "C" int vexb_jit_source_multi_dev(int dev, int lhs_dtype, int assign_op, int ncomp, const vexb_expr *const *exprs, char *buf,
+                                         size_t *len, int compile) {
+    VEXB_TRY(check_print_dev(dev));
     VEXB_CHECK(len && exprs, "NULL argument");
     VEXB_CHECK(ncomp >= 2 && ncomp <= 8, "a multi-expression kernel takes 2..8 components");
     VEXB_CHECK(lhs_dtype >= VEXB_F64 && lhs_dtype <= VEXB_U64, "bad lhs dtype %d", lhs_dtype);
@@ -1036,9 +1185,10 @@ extern "C" int vexb_jit_source_multi(int lhs_dtype, int assign_op, int ncomp, co
     }
     std::string src;
     VEXB_TRY(generate_source_n(ps.data(), ncomp, lhs_dtype, assign_op, &src));
+    src = with_program_header(header_for(dev, ps.data(), ncomp), src);
     if (compile) {
         std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log));
+        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(ps.data(), ncomp)));
         src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
     }
     if (buf) {
@@ -1050,6 +1200,11 @@ extern "C" int vexb_jit_source_multi(int lhs_dtype, int assign_op, int ncomp, co
 }
 
 extern "C" int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile) {
+    return vexb_jit_source_dev(-1, lhs_dtype, assign_op, expr, buf, len, compile);
+}
+
+extern "C" int vexb_jit_source_dev(int dev, int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile) {
+    VEXB_TRY(check_print_dev(dev));
     VEXB_CHECK(len, "len is NULL");
     VEXB_CHECK(lhs_dtype >= VEXB_F64 && lhs_dtype <= VEXB_U64, "bad lhs dtype %d", lhs_dtype);
     VEXB_CHECK(assign_op >= VEXB_SET && assign_op <= VEXB_RSH, "bad assign op %d", assign_op);
@@ -1057,9 +1212,11 @@ extern "C" int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *ex
     VEXB_TRY(normalize_expr(expr, &e, false));
     std::string src;
     VEXB_TRY(generate_source(e, lhs_dtype, assign_op, &src));
+    const vexb_expr *pe = &e;
+    src = with_program_header(header_for(dev, &pe, 1), src);
     if (compile) {
         std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log));
+        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(&pe, 1)));
         src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
         if (!log.empty()) src += "/* log:\n" + log + "*/\n";
     }
@@ -1075,6 +1232,12 @@ extern "C" int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *ex
 // `dtype`, as text (and, with compile != 0, compiled by NVRTC for sm_90a without touching a device).  The skeleton follows
 // the tunables in force ("eval.force_interp").  Every argument is checked before anything is generated.
 extern "C" int vexb_jit_source_reduce(int dtype, int nops, const int *ops, const vexb_expr *expr, char *buf, size_t *len, int compile) {
+    return vexb_jit_source_reduce_dev(-1, dtype, nops, ops, expr, buf, len, compile);
+}
+
+extern "C" int vexb_jit_source_reduce_dev(int dev, int dtype, int nops, const int *ops, const vexb_expr *expr, char *buf, size_t *len,
+                                          int compile) {
+    VEXB_TRY(check_print_dev(dev));
     VEXB_CHECK(len, "len is NULL");
     VEXB_CHECK(dtype >= VEXB_F64 && dtype <= VEXB_U64, "bad dtype %d", dtype);
     VEXB_CHECK(nops >= 1 && nops <= VEXB_MAX_COMBINED && ops, "between 1 and %d reductions can be combined", VEXB_MAX_COMBINED);
@@ -1088,9 +1251,11 @@ extern "C" int vexb_jit_source_reduce(int dtype, int nops, const int *ops, const
     VEXB_TRY(normalize_expr(expr, &e, false));
     std::string src;
     VEXB_TRY(generate_reduce_source(e, dtype, nops, mo, reduce_skeleton(e, dtype, nops > 1), &src));
+    const vexb_expr *pe = &e;
+    src = with_program_header(header_for(dev, &pe, 1), src);
     if (compile) {
         std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log));
+        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(&pe, 1)));
         src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
         if (!log.empty()) src += "/* log:\n" + log + "*/\n";
     }

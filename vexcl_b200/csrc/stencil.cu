@@ -400,7 +400,8 @@ extern "C" int vexb_stencil_operator_apply(int dev, void *stream, int id, const 
     VEXB_CHECK(n < ((size_t)1 << 38), "slice too long");
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     void *fn = nullptr;
-    VEXB_TRY(vexb::jit_build(dev, vexb::stencil_op_source(op), "vexb_stencil_op", &fn));
+    // the operator's body is user text: the device's program header goes first, and is part of the cache key (the text)
+    VEXB_TRY(vexb::jit_build(dev, vexb::with_program_header(vexb::program_header(dev), vexb::stencil_op_source(op)), "vexb_stencil_op", &fn));
     long long nn = (long long)n;
     double a64 = alpha; float a32 = (float)alpha;
     void *args[] = {&x, &nn, &left, &right, &y, op.dtype == VEXB_F64 ? (void *)&a64 : (void *)&a32, &append};
