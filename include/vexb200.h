@@ -99,6 +99,7 @@ typedef enum {
 #define VEXB_MAX_TERMS 16
 #define VEXB_MAX_CODE  64
 #define VEXB_MAX_STACK 12
+#define VEXB_MAX_TEMPS 8   /* temporary slots of one program (VEXB_OP_TDEF / VEXB_OP_TREF) */
 
 typedef enum {
     VEXB_TERM_VEC = 0,    /* v.ptr: device array of `dtype`, element i of this device slice */
@@ -167,13 +168,27 @@ typedef enum {
     VEXB_OP_CALL,     /* user function (VEX_FUNCTION): arg = id from vexb_function_register; pops its
                          declared number of arguments (already converted to the declared types), pushes
                          `type` = its return type.  Expressions with calls run on the NVRTC side path. */
+    /* Temporaries (vex::make_temp, vexcl/temporary.hpp): a subexpression evaluated once per element into a local
+     * variable that every use reads.  TDEF pops one value of `type` into temporary slot `arg` (< VEXB_MAX_TEMPS); it is
+     * legal only at stack depth 1 and leaves the stack empty, so every definition comes before the main expression (a
+     * program is: definitions in post-order, dependencies first, then the expression).  TREF pushes temporary `arg` with
+     * the type of its TDEF.  A temporary is evaluated for every element, whether or not a branch of a SELECT reads it,
+     * and the program has the bits of the same program with the definition written out at each TREF.  Refused with
+     * VEXB_ERR_INVALID by every entry point, before any launch or NVRTC run: a slot >= VEXB_MAX_TEMPS, a second TDEF of
+     * one slot, a TREF before its TDEF, a TREF whose type differs from its TDEF's, a TDEF whose type differs from the
+     * value on top of the stack, a TDEF at a depth other than 1.  vexb_eval and the reductions serve such programs with
+     * the interpreter or the generated kernel, never a hand-written sweep.  In vexb_eval_multi each component's slots
+     * are its own; a temporary that two components define by the same instructions over equal terminals (same kind,
+     * dtype and pointer or value) is computed once per element by the generated kernel and handed to both. */
+    VEXB_OP_TDEF,
+    VEXB_OP_TREF,
     VEXB_OP_COUNT_
 } vexb_opcode;
 
 typedef struct {
     uint8_t  op;    /* vexb_opcode */
     uint8_t  type;  /* vexb_dtype  */
-    uint16_t arg;   /* TERM: term slot; CVT: source dtype */
+    uint16_t arg;   /* TERM: term slot; CVT: source dtype; CALL: function id; TDEF / TREF: temporary slot */
 } vexb_instr;
 
 typedef struct {

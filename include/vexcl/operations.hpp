@@ -15,7 +15,9 @@
  * types follow C++'s usual arithmetic conversions; comparisons and logical operators
  * yield int.
  */
+#include <algorithm>
 #include <cstring>
+#include <string>
 #include <type_traits>
 #include <utility>
 #include <vector>
@@ -100,6 +102,52 @@ struct ir_builder {
         emit(VEXB_OP_TERM, dtype, k);
     }
     void cvt(int from, int to) { if (from != to) emit(VEXB_OP_CVT, to, from); }
+
+    // ---- temporaries (vex::make_temp, temporary.hpp) ----
+    // The program is code[0, n_prefix), the definitions in post-order (each ends with its VEXB_OP_TDEF), then the
+    // expression.  A definition is lowered in place, where its first use is, and then moved to the end of the prefix.
+    int n_prefix = 0;
+    struct temp_def { size_t tag; int type; std::string def; };
+    std::vector<temp_def> temps;                      ///< slot k: temporary make_temp<tag>, with its definition by content
+
+    /// A temporary whose definition was just lowered: code[n_prefix + rel, n_code), with terminals from slot `terms` on.
+    /// The first use of `tag` moves it into the prefix; a later one drops it again (when it is the same program) and both
+    /// read the one slot.
+    void use_temp(size_t tag, int rel, int terms, int type) {
+        const int from = n_prefix + rel;              // definitions of nested temporaries have moved into the prefix meanwhile
+        const std::string def = definition(from, e.n_code);
+        for (size_t k = 0; k < temps.size(); ++k) if (temps[k].tag == tag) {
+            if (temps[k].def != def || temps[k].type != type)
+                throw backend::error(VEXB_ERR_INVALID, "make_temp<" + std::to_string(tag) + ">: one tag names two different expressions");
+            e.n_code = from;                          // the same program: its second lowering (no new temporaries) goes
+            for (int j = terms; j < e.n_terms; ++j) std::memset(&e.term[j], 0, sizeof(vexb_term));
+            e.n_terms = terms;
+            emit(VEXB_OP_TREF, type, static_cast<int>(k));
+            return;
+        }
+        precondition(temps.size() < VEXB_MAX_TEMPS, "expression has too many temporaries");
+        emit(VEXB_OP_TDEF, type, static_cast<int>(temps.size()));
+        std::rotate(e.code + n_prefix, e.code + from, e.code + e.n_code);
+        n_prefix += e.n_code - from;
+        temps.push_back(temp_def{tag, type, def});
+        emit(VEXB_OP_TREF, type, static_cast<int>(temps.size() - 1));
+    }
+    private:
+        // code[from, to) with every terminal by content (a product's x too), so that two lowerings compare equal
+        std::string definition(int from, int to) const {
+            std::string d;
+            for (int pc = from; pc < to; ++pc) {
+                const vexb_instr &in = e.code[pc];
+                d.append(reinterpret_cast<const char*>(&in), sizeof(in) - sizeof(in.arg));
+                if (in.op != VEXB_OP_TERM) { d.append(reinterpret_cast<const char*>(&in.arg), sizeof(in.arg)); continue; }
+                vexb_term t = e.term[in.arg];
+                const bool product = t.kind == VEXB_TERM_SPMV || t.kind == VEXB_TERM_CCSR;
+                if (product) t.pad[0] = 0;
+                d.append(reinterpret_cast<const char*>(&t), sizeof(t));
+                if (product) d.append(reinterpret_cast<const char*>(&e.term[e.term[in.arg].pad[0]]), sizeof(vexb_term));
+            }
+            return d;
+        }
 };
 
 /// Queue list / partition / size of the first vector terminal (get_expression_properties, operations.hpp:1411).

@@ -15,6 +15,7 @@
 #include "element_index.hpp"
 #include "constants.hpp"
 #include "tagged_terminal.hpp"
+#include "temporary.hpp"
 #include "reductor.hpp"
 #include "spmat.hpp"
 #include "spmat/ccsr.hpp"

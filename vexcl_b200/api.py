@@ -328,6 +328,20 @@ class UserFunction:
         return Call(self, args)
 
 
+class Temp(Node):
+    """vex::make_temp<tag, T>(expr) (vexcl/temporary.hpp): `expr` evaluated once per element, before the expression that
+    uses it, into a local variable of `dtype` (expr's type by default) that every use reads.  Within one expression a tag
+    is one temporary; the same tag over a different expression is refused."""
+    def __init__(self, tag: int, expr, dtype=None):
+        self.tag, self.a = int(tag), wrap(expr)
+        self.dtype = self.a.dtype if dtype is None else _vdt(dtype)
+
+
+def make_temp(tag: int, expr, dtype=None) -> Temp:
+    """vex::make_temp<tag>(expr), or vex::make_temp<tag, dtype>(expr)."""
+    return Temp(tag, expr, dtype)
+
+
 def _header_devices(ctx: Context):
     return sorted(set(ctx.devs[k] for k in ctx.local))
 
@@ -387,6 +401,10 @@ class _Lowering:
         # launch is enqueued)
         self.target = None
         self.keep = []
+        # temporaries (Temp): code[0, n_prefix) holds their definitions, each ending with its TDEF; slot k of `temps` is
+        # (tag, dtype, definition by content, node)
+        self.n_prefix = 0
+        self.temps = []
 
     def term(self, kind, dtype, pad0: int = 0, **kw) -> int:
         k = self.e.n_terms
@@ -470,6 +488,8 @@ class _Lowering:
             for a, t in zip(n.args, n.fn.arg_types):
                 self.lower(a); self.cvt(a.dtype, t)
             self.emit("CALL", n.fn.ret, n.fn.id)
+        elif isinstance(n, Temp):
+            self.temp(n)
         elif isinstance(n, Select):
             self.lower(n.cond)
             if n.cond.dtype != L.I32:                     # any arithmetic condition: (c != 0)
@@ -480,6 +500,57 @@ class _Lowering:
             self.emit("SELECT", n.dtype)
         else:
             raise TypeError(f"cannot lower {type(n)}")
+
+    def temp(self, n: Temp):
+        """Lower the definition where the temporary is first used, then move it to the end of the prefix; a later use of
+        the tag drops its lowering again (when it is the same program) and reads the same slot."""
+        for k, (tag, typ, dk, node) in enumerate(self.temps):
+            if node is n:                       # the same node again: no second lowering (nor product temporary)
+                self.emit("TREF", n.dtype, k)
+                return
+        rel, terms = self.e.n_code - self.n_prefix, self.e.n_terms
+        self.lower(n.a)
+        self.cvt(n.a.dtype, n.dtype)
+        frm = self.n_prefix + rel               # nested temporaries have moved into the prefix meanwhile
+        d = self._definition(frm, self.e.n_code)
+        for k, (tag, typ, dk, node) in enumerate(self.temps):
+            if tag == n.tag:
+                if dk != d or typ != n.dtype:
+                    raise ValueError(f"make_temp({tag}): one tag names two different expressions")
+                self.e.n_code = frm
+                for j in range(terms, self.e.n_terms):
+                    C.memset(C.addressof(self.e.term[j]), 0, C.sizeof(L.Term))
+                self.e.n_terms = terms
+                self.emit("TREF", n.dtype, k)
+                return
+        if len(self.temps) >= L.MAX_TEMPS:
+            raise ValueError("expression has too many temporaries")
+        self.emit("TDEF", n.dtype, len(self.temps))
+        code = [(c.op, c.type, c.arg) for c in self.e.code[self.n_prefix:self.e.n_code]]
+        cut = frm - self.n_prefix
+        for j, (op, typ, arg) in enumerate(code[cut:] + code[:cut]):
+            ins = self.e.code[self.n_prefix + j]
+            ins.op, ins.type, ins.arg = op, typ, arg
+        self.n_prefix += self.e.n_code - frm
+        self.temps.append((n.tag, n.dtype, d, n))
+        self.emit("TREF", n.dtype, len(self.temps) - 1)
+
+    def _definition(self, frm, to) -> bytes:
+        """code[frm, to) with every terminal by content (a product's x too)."""
+        out = []
+        for pc in range(frm, to):
+            c = self.e.code[pc]
+            out.append(bytes((c.op, c.type)))
+            if c.op != L.OP["TERM"]:
+                out.append(c.arg.to_bytes(2, "little"))
+                continue
+            t = self.e.term[c.arg]
+            raw = bytearray(C.string_at(C.addressof(t), C.sizeof(L.Term)))
+            if t.kind in (L.TERM_SPMV, L.TERM_CCSR):
+                raw[2] = 0
+                raw += C.string_at(C.addressof(self.e.term[t.pad[0]]), C.sizeof(L.Term))
+            out.append(bytes(raw))
+        return b"".join(out)
 
 
 def _has_call(n) -> bool:

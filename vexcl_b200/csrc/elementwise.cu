@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(256) sweep_kernel(T *lhs, SweepArgs a, size_t 
     }
 }
 
-template <int U>
+template <int U, bool TEMPS>
 __global__ void __launch_bounds__(256) interp_kernel(const __grid_constant__ vexb_expr e, void *lhs, int lhs_dtype,
                                                       size_t n, size_t index_offset) {
     const int rt = program_result_type(e);
@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) interp_kernel(const __grid_constant__ vex
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int k = 0; k < U; ++k) { idx[k] = base + (size_t)k * blockDim.x + threadIdx.x; active[k] = idx[k] < n; }
-        eval_expr<U>(e, idx, active, index_offset, out);
+        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int k = 0; k < U; ++k)
             if (active[k]) store_as(lhs, idx[k], convert(out[k], rt, lhs_dtype), lhs_dtype);
@@ -168,9 +168,11 @@ static int fold_compound(const vexb_expr &e, const void *lhs, int lhs_dtype, int
     vexb_term &lt = out->term[e.n_terms];
     lt.kind = VEXB_TERM_VEC; lt.dtype = (uint8_t)lhs_dtype; lt.v.ptr = lhs;
     int n = 0;
+    const int defs = temp_prefix_length(e);                 // temporaries are defined on an empty stack: before lhs[i]
+    for (int pc = 0; pc < defs; ++pc) out->code[n++] = e.code[pc];
     out->code[n++] = vexb_instr{VEXB_OP_TERM, (uint8_t)lhs_dtype, (uint16_t)e.n_terms};
     if (lhs_dtype != C) out->code[n++] = vexb_instr{VEXB_OP_CVT, (uint8_t)C, (uint16_t)lhs_dtype};
-    for (int pc = 0; pc < e.n_code; ++pc) out->code[n++] = e.code[pc];
+    for (int pc = defs; pc < e.n_code; ++pc) out->code[n++] = e.code[pc];
     if (R != C) out->code[n++] = vexb_instr{VEXB_OP_CVT, (uint8_t)C, (uint16_t)R};
     out->code[n++] = vexb_instr{(uint8_t)opmap[aop], (uint8_t)C, 0};
     out->n_code = n;
@@ -242,7 +244,8 @@ extern "C" int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int as
     size_t want = (n + per_block - 1) / per_block;
     const size_t cap = (size_t)sms * (size_t)param("interp.blocks_per_sm", 4);
     const int blocks = (int)(want < cap ? want : cap);
-    interp_kernel<4><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
+    if (expr_has_temps(prog)) interp_kernel<4, true><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
+    else                      interp_kernel<4, false><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
     VEXB_LAUNCHED();
     return VEXB_OK;
 }

@@ -235,10 +235,15 @@ __host__ __device__ inline int program_result_type(const vexb_expr &e) {
 // Evaluate the program for U element indices at once (U independent lanes give
 // the memory system U loads in flight per terminal).  The top of the stack is
 // kept in registers; deeper entries spill to a small per-thread array.
-template <int U>
+// TEMPS: the program may define temporaries (VEXB_OP_TDEF / VEXB_OP_TREF), kept in
+// a per-lane file beside the stack.  Programs without them take the TEMPS = false
+// instantiation, which is exactly the evaluator without those arms: two more arms in
+// the one switch cost the 32-bit reductions register spills they did not have.
+template <int U, bool TEMPS = false>
 __device__ __forceinline__ void eval_expr(const vexb_expr &e, const size_t (&idx)[U], const bool (&active)[U],
                                           size_t index_offset, V (&out)[U]) {
     V st[VEXB_MAX_STACK][U];
+    V tmp[TEMPS ? VEXB_MAX_TEMPS : 1][U];
     V tos[U];
     int d = 0;
 #pragma unroll
@@ -250,6 +255,19 @@ __device__ __forceinline__ void eval_expr(const vexb_expr &e, const size_t (&idx
     for (int pc = 0; pc < n_code; ++pc) {
         const vexb_instr in = e.code[pc];
         const int op = in.op, t = in.type;
+        if constexpr (TEMPS) {
+            if (op == VEXB_OP_TDEF) {           // the host admits it at depth 1 only: the stack is empty after it
+                VEXB_LANES tmp[in.arg][k] = tos[k];
+                d = 0;
+                continue;
+            }
+            if (op == VEXB_OP_TREF) {
+                if (d > 0) { VEXB_LANES st[d - 1][k] = tos[k]; }
+                VEXB_LANES tos[k] = tmp[in.arg][k];
+                ++d;
+                continue;
+            }
+        }
         switch (op) {
             case VEXB_OP_TERM: {
                 if (d > 0) { VEXB_LANES st[d - 1][k] = tos[k]; }

@@ -20,6 +20,8 @@ inline int op_arity(int op) {
     if (op == VEXB_OP_SELECT || op == VEXB_OP_FMA) return 3;
     if (op >= VEXB_OP_SIN && op <= VEXB_OP_TRUNC) return 1;
     if (op >= VEXB_OP_POW && op <= VEXB_OP_FMAX) return 2;
+    if (op == VEXB_OP_TDEF) return 1;
+    if (op == VEXB_OP_TREF) return 0;
     return -1;
 }
 
@@ -85,6 +87,18 @@ inline bool expr_has_call(const vexb_expr &e) {
     return false;
 }
 
+inline bool expr_has_temps(const vexb_expr &e) {
+    for (int pc = 0; pc < e.n_code; ++pc) if (e.code[pc].op == VEXB_OP_TDEF) return true;
+    return false;
+}
+
+// Number of leading instructions that define temporaries: the program up to and including its last TDEF (0 without).
+inline int temp_prefix_length(const vexb_expr &e) {
+    int n = 0;
+    for (int pc = 0; pc < e.n_code; ++pc) if (e.code[pc].op == VEXB_OP_TDEF) n = pc + 1;
+    return n;
+}
+
 inline int host_result_type(const vexb_expr &e) {
     if (e.n_code <= 0) return VEXB_F64;
     const vexb_instr &in = e.code[e.n_code - 1];
@@ -125,6 +139,11 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     for (int k = 0; k < VEXB_MAX_TERMS; ++k) remap[k] = -1;
     memset(out, 0, sizeof(*out));
     int depth = 0, maxdepth = 0;
+    // temporaries: the type each slot was defined with (-1: not yet), and the type of every value on the stack (the TDEF
+    // check needs the top's)
+    int temp_type[VEXB_MAX_TEMPS];
+    for (int k = 0; k < VEXB_MAX_TEMPS; ++k) temp_type[k] = -1;
+    int stype[VEXB_MAX_CODE + 1];
     for (int pc = 0; pc < in->n_code; ++pc) {
         vexb_instr ins = in->code[pc];
         int ar = op_arity(ins.op);
@@ -136,6 +155,23 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
         VEXB_CHECK(ar >= 0, "instr %d: unknown opcode %d", pc, (int)ins.op);
         VEXB_CHECK(ins.type <= VEXB_U64, "instr %d: bad type %d", pc, (int)ins.type);
         VEXB_CHECK(depth >= ar, "instr %d: stack underflow", pc);
+        if (ins.op == VEXB_OP_TDEF || ins.op == VEXB_OP_TREF) {
+            VEXB_CHECK(ins.arg < VEXB_MAX_TEMPS, "instr %d: temporary slot %d out of range (at most %d temporaries)", pc, (int)ins.arg, VEXB_MAX_TEMPS);
+            if (ins.op == VEXB_OP_TDEF) {
+                VEXB_CHECK(temp_type[ins.arg] < 0, "instr %d: temporary %d is defined twice", pc, (int)ins.arg);
+                VEXB_CHECK(depth == 1, "instr %d: a temporary is defined at stack depth %d (definitions come first, at depth 1)", pc, depth);
+                VEXB_CHECK(stype[0] == ins.type, "instr %d: temporary %d has type %d, the value it stores type %d", pc, (int)ins.arg, (int)ins.type, stype[0]);
+                temp_type[ins.arg] = ins.type;
+                depth = 0;
+            } else {
+                VEXB_CHECK(temp_type[ins.arg] >= 0, "instr %d: temporary %d is read before its definition", pc, (int)ins.arg);
+                VEXB_CHECK(temp_type[ins.arg] == ins.type, "instr %d: temporary %d is read as type %d, defined as type %d", pc, (int)ins.arg, (int)ins.type, temp_type[ins.arg]);
+                stype[depth++] = ins.type;
+                if (depth > maxdepth) maxdepth = depth;
+            }
+            out->code[out->n_code++] = ins;
+            continue;
+        }
         if (ins.op == VEXB_OP_TERM) {
             VEXB_CHECK(ins.arg < in->n_terms, "instr %d: term slot %d out of range", pc, (int)ins.arg);
             const vexb_term &t = in->term[ins.arg];
@@ -191,6 +227,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
                         prev.arg = (uint16_t)slot;
                     }
                     prev.type = ins.type;
+                    stype[depth - 1] = ins.type;
                     continue;
                 }
             }
@@ -203,6 +240,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
         }
         depth += 1 - ar;
         if (depth > maxdepth) maxdepth = depth;
+        stype[depth - 1] = ((ins.op >= VEXB_OP_LT && ins.op <= VEXB_OP_LOR) || ins.op == VEXB_OP_LNOT) ? VEXB_I32 : ins.type;
         out->code[out->n_code++] = ins;
     }
     VEXB_CHECK(depth == 1, "program leaves %d values on the stack (expected 1)", depth);

@@ -13,6 +13,7 @@
 #include "peer.cuh"
 #include "fold_text.inc"       // kFoldText: csrc/fold.cuh byte for byte, stringified by vexcl_b200/build.py
 #include <dlfcn.h>
+#include <algorithm>
 #include <cctype>
 #include <map>
 #include <mutex>
@@ -179,6 +180,154 @@ static int sell_sweep_term(const vexb_expr &e, int *term) {
     return VEXB_OK;
 }
 
+// Print instructions [from, to) of a normalised program as CUDA C onto the value stack `st`: one `const T rPC = ...;` per
+// instruction, whose semantics mirror csrc/expr_eval.cuh.  A TDEF prints `const T tK = <top>;` and names slot K tK; a
+// TREF pushes tnames[K], which is tK or the parameter that carries the value in (multi-expression kernels).
+static void print_code(const vexb_expr &e, int from, int to, std::string (&tnames)[VEXB_MAX_TEMPS], std::ostream &s,
+                       std::vector<std::pair<std::string, int>> &st) {
+    for (int pc = from; pc < to; ++pc) {
+        const vexb_instr &in = e.code[pc];
+        const int op = in.op, t = in.type;
+        std::ostringstream r;
+        int rt = t;
+        auto pop = [&]() { auto v = st.back(); st.pop_back(); return v; };
+        if (op == VEXB_OP_TDEF) {
+            tnames[in.arg] = "t" + std::to_string(in.arg);
+            s << "    const " << ctype(t) << " " << tnames[in.arg] << " = " << pop().first << ";\n";
+            continue;
+        }
+        if (op == VEXB_OP_TREF) { st.emplace_back(tnames[in.arg], t); continue; }
+        if (op == VEXB_OP_TERM) {
+            const vexb_term &tm = e.term[in.arg];
+            const int k = in.arg;
+            rt = tm.kind == VEXB_TERM_INDEX ? VEXB_U64 : tm.dtype;
+            if (tm.kind == VEXB_TERM_VEC) r << "__ldcs((const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr + i)";
+            else if (tm.kind == VEXB_TERM_DSCALAR) r << "*(const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr";
+            else if (tm.kind == VEXB_TERM_SPMV) r << "spmv_" << k << "((const spmv_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
+                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i"
+                                                  << (static_cast<const vexb_spmat *>(tm.v.ptr)->fmt == VEXB_FMT_SELL ? ", t)" : ")");
+            else if (tm.kind == VEXB_TERM_CCSR) r << "ccsr_" << k << "((const ccsr_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
+                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i)";
+            else if (tm.kind == VEXB_TERM_SCALAR) r << "tt.t[" << k << "].v." << ufield(rt);
+            else r << "off + i + (unsigned long long)tt.t[" << k << "].v.i64";
+        } else if (op == VEXB_OP_CVT) {
+            auto a = pop(); r << "(" << ctype(t) << ")" << a.first;
+        } else if (op == VEXB_OP_NEG) {
+            auto a = pop(); r << "-" << a.first;
+        } else if (op == VEXB_OP_LNOT) {
+            auto a = pop(); rt = VEXB_I32; r << "(int)!" << a.first;
+        } else if (op == VEXB_OP_SELECT) {
+            auto c = pop(), b = pop(), a = pop();
+            r << "(" << a.first << " != 0) ? " << b.first << " : " << c.first;
+        } else if (op == VEXB_OP_FMA) {
+            auto c = pop(), b = pop(), a = pop();
+            r << (t == VEXB_F32 ? "fmaf(" : "fma(") << a.first << ", " << b.first << ", " << c.first << ")";
+        } else if (op == VEXB_OP_CALL) {
+            std::vector<std::string> args(function_arity(in.arg));
+            for (int k = (int)args.size() - 1; k >= 0; --k) args[k] = pop().first;
+            std::string nm; { std::lock_guard<std::mutex> l(g_fmx); nm = g_funcs[in.arg].name; }
+            r << nm << "_" << in.arg << "(";
+            for (size_t k = 0; k < args.size(); ++k) r << (k ? ", " : "") << args[k];
+            r << ")";
+        } else if ((op >= VEXB_OP_ADD && op <= VEXB_OP_LOR) || (op >= VEXB_OP_POW && op <= VEXB_OP_FMAX)) {
+            auto b = pop(), a = pop();
+            const std::string &x = a.first, &y = b.first;
+            const int bits = (t == VEXB_I32 || t == VEXB_U32) ? 31 : 63;
+            switch (op) {
+                case VEXB_OP_ADD: r << x << " + " << y; break;
+                case VEXB_OP_SUB: r << x << " - " << y; break;
+                case VEXB_OP_MUL: r << x << " * " << y; break;
+                case VEXB_OP_DIV:
+                    if (is_f(t)) r << x << " / " << y;
+                    else if (is_signed(t)) r << "(" << y << " == 0) ? 0 : (" << y << " == -1 ? (" << ctype(t) << ")(0 - (unsigned " << (t == VEXB_I32 ? "int" : "long long") << ")" << x << ") : " << x << " / " << y << ")";
+                    else r << "(" << y << " == 0) ? 0 : " << x << " / " << y;
+                    break;
+                case VEXB_OP_MOD: case VEXB_OP_FMOD:
+                    if (is_f(t)) r << (t == VEXB_F32 ? "fmodf(" : "fmod(") << x << ", " << y << ")";
+                    else if (is_signed(t)) r << "(" << y << " == 0 || " << y << " == -1) ? 0 : " << x << " % " << y;
+                    else r << "(" << y << " == 0) ? 0 : " << x << " % " << y;
+                    break;
+                case VEXB_OP_BAND: r << x << " & " << y; break;
+                case VEXB_OP_BOR:  r << x << " | " << y; break;
+                case VEXB_OP_BXOR: r << x << " ^ " << y; break;
+                case VEXB_OP_SHL:  r << x << " << (" << y << " & " << bits << ")"; break;
+                case VEXB_OP_SHR:  r << x << " >> (" << y << " & " << bits << ")"; break;
+                case VEXB_OP_LT: rt = VEXB_I32; r << "(int)(" << x << " < " << y << ")"; break;
+                case VEXB_OP_GT: rt = VEXB_I32; r << "(int)(" << x << " > " << y << ")"; break;
+                case VEXB_OP_LE: rt = VEXB_I32; r << "(int)(" << x << " <= " << y << ")"; break;
+                case VEXB_OP_GE: rt = VEXB_I32; r << "(int)(" << x << " >= " << y << ")"; break;
+                case VEXB_OP_EQ: rt = VEXB_I32; r << "(int)(" << x << " == " << y << ")"; break;
+                case VEXB_OP_NE: rt = VEXB_I32; r << "(int)(" << x << " != " << y << ")"; break;
+                case VEXB_OP_LAND: rt = VEXB_I32; r << "(int)((" << x << " != 0) && (" << y << " != 0))"; break;
+                case VEXB_OP_LOR:  rt = VEXB_I32; r << "(int)((" << x << " != 0) || (" << y << " != 0))"; break;
+                case VEXB_OP_FMIN: case VEXB_OP_FMAX:
+                    if (is_f(t)) r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << x << ", " << y << ")";
+                    else r << "(" << x << (op == VEXB_OP_FMIN ? " < " : " > ") << y << ") ? " << x << " : " << y;
+                    break;
+                default: r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << x << ", " << y << ")"; break;
+            }
+        } else {    // unary math
+            auto a = pop();
+            if (op == VEXB_OP_FABS && !is_f(t)) {
+                if (is_signed(t)) r << "(" << a.first << " < 0) ? (" << ctype(t) << ")(0 - (unsigned " << (t == VEXB_I32 ? "int" : "long long") << ")" << a.first << ") : " << a.first;
+                else r << a.first;
+            } else r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << a.first << ")";
+        }
+        std::string name = "r" + std::to_string(pc);
+        s << "    const " << ctype(rt) << " " << name << " = " << r.str() << ";\n";
+        st.emplace_back(name, rt);
+    }
+}
+
+// The temporaries of a multi-expression assignment.  Each component's slots are its own; a temporary that several
+// components define by the same instructions over equal terminals (same kind, dtype and pointer or value) is one class,
+// which the kernel computes once per element and hands to every component that reads it (`vex::tie(a, b) =
+// std::tie(t, sqrt(1 - t*t))` evaluates t once).  Classes are numbered in the order components define them, so a class
+// comes after the classes its definition reads.
+struct TempClasses {
+    int cls[8][VEXB_MAX_TEMPS];                         // class of component c's slot k, -1 where c does not define k
+    std::vector<int> comp, from, to, type;              // class g: defined by instructions [from, to) of component comp
+    std::vector<std::vector<int>> reads;                // class g: the classes its definition reads, in order of first use
+};
+
+static TempClasses temp_classes(const vexb_expr *const *es, int ncomp) {
+    TempClasses tc;
+    std::vector<std::string> keys;
+    for (int c = 0; c < ncomp; ++c) {
+        const vexb_expr &e = *es[c];
+        for (int k = 0; k < VEXB_MAX_TEMPS; ++k) tc.cls[c][k] = -1;
+        std::string key;                                // the definition of the next TDEF, terminals by content
+        int from = 0;
+        for (int pc = 0; pc < e.n_code; ++pc) {
+            const vexb_instr &in = e.code[pc];
+            if (in.op == VEXB_OP_TDEF) {
+                key.push_back((char)in.type);
+                int g = 0;
+                while (g < (int)keys.size() && keys[g] != key) ++g;
+                if (g == (int)keys.size()) {
+                    keys.push_back(key);
+                    tc.comp.push_back(c); tc.from.push_back(from); tc.to.push_back(pc); tc.type.push_back(in.type);
+                    std::vector<int> reads;
+                    for (int q = from; q < pc; ++q) if (e.code[q].op == VEXB_OP_TREF) {
+                        const int j = tc.cls[c][e.code[q].arg];
+                        if (std::find(reads.begin(), reads.end(), j) == reads.end()) reads.push_back(j);
+                    }
+                    tc.reads.push_back(reads);
+                }
+                tc.cls[c][in.arg] = g;
+                key.clear();
+                from = pc + 1;
+                continue;
+            }
+            key.push_back((char)in.op); key.push_back((char)in.type);
+            if (in.op == VEXB_OP_TERM) key.append(reinterpret_cast<const char *>(&e.term[in.arg]), sizeof(vexb_term));
+            else if (in.op == VEXB_OP_TREF) key += "#" + std::to_string(tc.cls[c][in.arg]);
+            else { key.push_back((char)(in.arg & 0xff)); key.push_back((char)(in.arg >> 8)); }
+        }
+    }
+    return tc;
+}
+
 // sell: where the terminal of the request's sliced-ELL strip goes (sell_sweep_term); NULL for the callers that do not
 // sweep in storage order (reductions), which refuse such strips.
 static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtype, int aop, std::ostringstream &s, bool *spmv, int *sell = nullptr) {
@@ -313,99 +462,39 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
              "  }\n  return sum;\n}\n";
     }
     const char *LT = ctype(lhs_dtype);
+    // Multi-expression kernels with temporaries: one function per class of temporaries (temp_classes), vexb_temp_g, which
+    // takes the classes its definition reads as parameters g<j>; the kernel calls each once per element and passes the
+    // values to the components, whose functions then start after their definitions.
+    bool multi_temps = false;
+    for (int comp = 0; ncomp > 1 && comp < ncomp; ++comp) multi_temps = multi_temps || expr_has_temps(*es[comp]);
+    const TempClasses tc = multi_temps ? temp_classes(es, ncomp) : TempClasses();
+    for (size_t g = 0; g < tc.comp.size(); ++g) {
+        const vexb_expr &e = *es[tc.comp[g]];
+        std::string tnames[VEXB_MAX_TEMPS];
+        for (int pc = tc.from[g]; pc < tc.to[g]; ++pc)
+            if (e.code[pc].op == VEXB_OP_TREF) tnames[e.code[pc].arg] = "g" + std::to_string(tc.cls[tc.comp[g]][e.code[pc].arg]);
+        s << "__device__ __forceinline__ " << ctype(tc.type[g]) << " vexb_temp_" << g << "(const terms_j &tt, unsigned long long i, unsigned long long off";
+        for (int j : tc.reads[g]) s << ", const " << ctype(tc.type[j]) << " g" << j;
+        s << ") {\n";
+        std::vector<std::pair<std::string, int>> st;
+        print_code(e, tc.from[g], tc.to[g], tnames, s, st);
+        VEXB_CHECK(st.size() == 1, "internal: a temporary did not reduce to one value");
+        s << "    return " << st.back().first << ";\n}\n";
+    }
     // One element of the assignment as a function; the kernel below evaluates four of them (a grid stride apart) before it
     // stores any, so a thread has 4 x (number of vector operands) loads in flight instead of one round trip per element.
     for (int comp = 0; comp < ncomp; ++comp) {
     const vexb_expr &e = *es[comp];
     s << "__device__ __forceinline__ " << LT << " vexb_elem" << (ncomp > 1 ? "_" + std::to_string(comp) : std::string()) << "(const terms_j &tt, const " << LT
-      << " *lhs, unsigned long long i, unsigned long long off" << (sweep ? ", unsigned long long t" : "") << ") {\n";
-    std::vector<std::pair<std::string, int>> st;        // (variable name, dtype)
-    for (int pc = 0; pc < e.n_code; ++pc) {
-        const vexb_instr &in = e.code[pc];
-        const int op = in.op, t = in.type;
-        std::ostringstream r;
-        int rt = t;
-        auto pop = [&]() { auto v = st.back(); st.pop_back(); return v; };
-        if (op == VEXB_OP_TERM) {
-            const vexb_term &tm = e.term[in.arg];
-            const int k = in.arg;
-            rt = tm.kind == VEXB_TERM_INDEX ? VEXB_U64 : tm.dtype;
-            if (tm.kind == VEXB_TERM_VEC) r << "__ldcs((const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr + i)";
-            else if (tm.kind == VEXB_TERM_DSCALAR) r << "*(const " << ctype(rt) << " *)tt.t[" << k << "].v.ptr";
-            else if (tm.kind == VEXB_TERM_SPMV) r << "spmv_" << k << "((const spmv_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
-                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i"
-                                                  << (static_cast<const vexb_spmat *>(tm.v.ptr)->fmt == VEXB_FMT_SELL ? ", t)" : ")");
-            else if (tm.kind == VEXB_TERM_CCSR) r << "ccsr_" << k << "((const ccsr_desc_j *)tt.t[" << k << "].v.ptr, (const " << ctype(rt)
-                                                  << " *)tt.t[" << (int)tm.pad[0] << "].v.ptr, i)";
-            else if (tm.kind == VEXB_TERM_SCALAR) r << "tt.t[" << k << "].v." << ufield(rt);
-            else r << "off + i + (unsigned long long)tt.t[" << k << "].v.i64";
-        } else if (op == VEXB_OP_CVT) {
-            auto a = pop(); r << "(" << ctype(t) << ")" << a.first;
-        } else if (op == VEXB_OP_NEG) {
-            auto a = pop(); r << "-" << a.first;
-        } else if (op == VEXB_OP_LNOT) {
-            auto a = pop(); rt = VEXB_I32; r << "(int)!" << a.first;
-        } else if (op == VEXB_OP_SELECT) {
-            auto c = pop(), b = pop(), a = pop();
-            r << "(" << a.first << " != 0) ? " << b.first << " : " << c.first;
-        } else if (op == VEXB_OP_FMA) {
-            auto c = pop(), b = pop(), a = pop();
-            r << (t == VEXB_F32 ? "fmaf(" : "fma(") << a.first << ", " << b.first << ", " << c.first << ")";
-        } else if (op == VEXB_OP_CALL) {
-            std::vector<std::string> args(function_arity(in.arg));
-            for (int k = (int)args.size() - 1; k >= 0; --k) args[k] = pop().first;
-            std::string nm; { std::lock_guard<std::mutex> l(g_fmx); nm = g_funcs[in.arg].name; }
-            r << nm << "_" << in.arg << "(";
-            for (size_t k = 0; k < args.size(); ++k) r << (k ? ", " : "") << args[k];
-            r << ")";
-        } else if ((op >= VEXB_OP_ADD && op <= VEXB_OP_LOR) || (op >= VEXB_OP_POW && op <= VEXB_OP_FMAX)) {
-            auto b = pop(), a = pop();
-            const std::string &x = a.first, &y = b.first;
-            const int bits = (t == VEXB_I32 || t == VEXB_U32) ? 31 : 63;
-            switch (op) {
-                case VEXB_OP_ADD: r << x << " + " << y; break;
-                case VEXB_OP_SUB: r << x << " - " << y; break;
-                case VEXB_OP_MUL: r << x << " * " << y; break;
-                case VEXB_OP_DIV:
-                    if (is_f(t)) r << x << " / " << y;
-                    else if (is_signed(t)) r << "(" << y << " == 0) ? 0 : (" << y << " == -1 ? (" << ctype(t) << ")(0 - (unsigned " << (t == VEXB_I32 ? "int" : "long long") << ")" << x << ") : " << x << " / " << y << ")";
-                    else r << "(" << y << " == 0) ? 0 : " << x << " / " << y;
-                    break;
-                case VEXB_OP_MOD: case VEXB_OP_FMOD:
-                    if (is_f(t)) r << (t == VEXB_F32 ? "fmodf(" : "fmod(") << x << ", " << y << ")";
-                    else if (is_signed(t)) r << "(" << y << " == 0 || " << y << " == -1) ? 0 : " << x << " % " << y;
-                    else r << "(" << y << " == 0) ? 0 : " << x << " % " << y;
-                    break;
-                case VEXB_OP_BAND: r << x << " & " << y; break;
-                case VEXB_OP_BOR:  r << x << " | " << y; break;
-                case VEXB_OP_BXOR: r << x << " ^ " << y; break;
-                case VEXB_OP_SHL:  r << x << " << (" << y << " & " << bits << ")"; break;
-                case VEXB_OP_SHR:  r << x << " >> (" << y << " & " << bits << ")"; break;
-                case VEXB_OP_LT: rt = VEXB_I32; r << "(int)(" << x << " < " << y << ")"; break;
-                case VEXB_OP_GT: rt = VEXB_I32; r << "(int)(" << x << " > " << y << ")"; break;
-                case VEXB_OP_LE: rt = VEXB_I32; r << "(int)(" << x << " <= " << y << ")"; break;
-                case VEXB_OP_GE: rt = VEXB_I32; r << "(int)(" << x << " >= " << y << ")"; break;
-                case VEXB_OP_EQ: rt = VEXB_I32; r << "(int)(" << x << " == " << y << ")"; break;
-                case VEXB_OP_NE: rt = VEXB_I32; r << "(int)(" << x << " != " << y << ")"; break;
-                case VEXB_OP_LAND: rt = VEXB_I32; r << "(int)((" << x << " != 0) && (" << y << " != 0))"; break;
-                case VEXB_OP_LOR:  rt = VEXB_I32; r << "(int)((" << x << " != 0) || (" << y << " != 0))"; break;
-                case VEXB_OP_FMIN: case VEXB_OP_FMAX:
-                    if (is_f(t)) r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << x << ", " << y << ")";
-                    else r << "(" << x << (op == VEXB_OP_FMIN ? " < " : " > ") << y << ") ? " << x << " : " << y;
-                    break;
-                default: r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << x << ", " << y << ")"; break;
-            }
-        } else {    // unary math
-            auto a = pop();
-            if (op == VEXB_OP_FABS && !is_f(t)) {
-                if (is_signed(t)) r << "(" << a.first << " < 0) ? (" << ctype(t) << ")(0 - (unsigned " << (t == VEXB_I32 ? "int" : "long long") << ")" << a.first << ") : " << a.first;
-                else r << a.first;
-            } else r << math_name(op) << (t == VEXB_F32 ? "f(" : "(") << a.first << ")";
-        }
-        std::string name = "r" + std::to_string(pc);
-        s << "    const " << ctype(rt) << " " << name << " = " << r.str() << ";\n";
-        st.emplace_back(name, rt);
+      << " *lhs, unsigned long long i, unsigned long long off" << (sweep ? ", unsigned long long t" : "");
+    std::string tnames[VEXB_MAX_TEMPS];
+    for (int k = 0; multi_temps && k < VEXB_MAX_TEMPS; ++k) if (tc.cls[comp][k] >= 0) {
+        tnames[k] = "t" + std::to_string(k);
+        s << ", const " << ctype(tc.type[tc.cls[comp][k]]) << " " << tnames[k];
     }
+    s << ") {\n";
+    std::vector<std::pair<std::string, int>> st;        // (variable name, dtype)
+    print_code(e, multi_temps ? temp_prefix_length(e) : 0, e.n_code, tnames, s, st);
     VEXB_CHECK(st.size() == 1, "internal: program did not reduce to one value");
     const std::string res = st.back().first; const int R = st.back().second;
     if (aop == VEXB_SET) {
@@ -453,7 +542,19 @@ static int generate_source_n(const vexb_expr *const *es, int ncomp, int lhs_dtyp
              "extern \"C\" __global__ void __launch_bounds__(256) vexb_jit_kernel(const multi_j mt, unsigned long long n, unsigned long long off) {\n"
              "  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;\n"
              "  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {\n";
-        for (int c = 0; c < ncomp; ++c) s << "    const " << LT << " a" << c << " = vexb_elem_" << c << "(mt.c[" << c << "], mt.lhs[" << c << "], i, off);\n";
+        bool temps = false;
+        for (int c = 0; c < ncomp; ++c) temps = temps || expr_has_temps(*es[c]);
+        const TempClasses tc = temps ? temp_classes(es, ncomp) : TempClasses();
+        for (size_t g = 0; g < tc.comp.size(); ++g) {
+            s << "    const " << ctype(tc.type[g]) << " g" << g << " = vexb_temp_" << g << "(mt.c[" << tc.comp[g] << "], i, off";
+            for (int j : tc.reads[g]) s << ", g" << j;
+            s << ");\n";
+        }
+        for (int c = 0; c < ncomp; ++c) {
+            s << "    const " << LT << " a" << c << " = vexb_elem_" << c << "(mt.c[" << c << "], mt.lhs[" << c << "], i, off";
+            for (int k = 0; temps && k < VEXB_MAX_TEMPS; ++k) if (tc.cls[c][k] >= 0) s << ", g" << tc.cls[c][k];
+            s << ");\n";
+        }
         for (int c = 0; c < ncomp; ++c) s << "    mt.lhs[" << c << "][i] = a" << c << ";\n";
         s << "  }\n}\n";
         *out = s.str();
@@ -895,6 +996,13 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
         for (int k = 0; k < es[c]->n_terms; ++k) if (is_product_term(es[c]->term[k].kind)) return VEXB_OK;
     std::string key(1, (char)ncomp);
     for (int c = 0; c < ncomp; ++c) { key += request_signature(*es[c], lhs_dtype, aop); key.push_back('|'); }
+    bool temps = false;
+    for (int c = 0; c < ncomp; ++c) temps = temps || expr_has_temps(*es[c]);
+    if (temps) {                                                      // which temporaries the components share: by pointer
+        const TempClasses tc = temp_classes(es, ncomp);
+        key += "temps:";
+        for (int c = 0; c < ncomp; ++c) for (int k = 0; k < VEXB_MAX_TEMPS; ++k) key.push_back((char)tc.cls[c][k]);
+    }
     const std::string header = header_for(dev, es, ncomp);
     std::shared_ptr<JitEntry> en;
     {

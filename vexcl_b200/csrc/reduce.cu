@@ -174,7 +174,7 @@ template <> __device__ __forceinline__ unsigned v_as<unsigned>(V v) { return (un
 template <> __device__ __forceinline__ long long v_as<long long>(V v) { return v.i; }
 template <> __device__ __forceinline__ unsigned long long v_as<unsigned long long>(V v) { return v.u; }
 
-template <int OP, class T, int U>
+template <int OP, class T, int U, bool TEMPS>
 __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constant__ vexb_expr e, int dtype, size_t n,
                                                              size_t index_offset, void *ws, T *result, PeerArgs pa) {
     const int rt = program_result_type(e);
@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constan
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int k = 0; k < U; ++k) { idx[k] = base + (size_t)k * blockDim.x + threadIdx.x; active[k] = idx[k] < n; }
-        eval_expr<U>(e, idx, active, index_offset, out);
+        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int k = 0; k < U; ++k) if (active[k]) acc[k].take(v_as<T>(convert(out[k], rt, dtype)));
     }
@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constan
 // the GPUs).
 struct MultiOps { int n; int op[VEXB_MAX_COMBINED]; };
 
-template <class T, int U>
+template <class T, int U, bool TEMPS>
 __global__ void __launch_bounds__(256) reduce_multi_kernel(const __grid_constant__ vexb_expr e, int dtype, size_t n, size_t index_offset,
                                                             MultiOps ops, void *ws, size_t ws_stride, T *result, PeerArgs pa) {
     const int rt = program_result_type(e);
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(256) reduce_multi_kernel(const __grid_constant
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) { idx[u] = base + (size_t)u * blockDim.x + threadIdx.x; active[u] = idx[u] < n; }
-        eval_expr<U>(e, idx, active, index_offset, out);
+        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int u = 0; u < U; ++u) if (active[u]) {
             const T v = v_as<T>(convert(out[u], rt, dtype));
@@ -262,7 +262,10 @@ static bool launch_rsweep_shape(int sh, int op, int blocks, cudaStream_t st, con
 template <class T>
 static void launch_rinterp(int op, int blocks, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t off, void *ws, void *res, const PeerArgs &pa) {
     switch (op) {
-#define C(OP) case OP: reduce_interp_kernel<OP, T, 4><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); break;
+#define C(OP) case OP: \
+        if (expr_has_temps(e)) reduce_interp_kernel<OP, T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); \
+        else                   reduce_interp_kernel<OP, T, 4, false><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); \
+        break;
         C(VEXB_SUM) C(VEXB_SUM_KAHAN) C(VEXB_MAX) C(VEXB_MIN) C(VEXB_MINMAX)
 #undef C
     }
@@ -426,7 +429,8 @@ extern "C" int vexb_cg_update_xp(int dev, void *stream, int dtype, size_t n, voi
 template <class T>
 static void launch_rmulti(int blocks, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t off, const vexb::MultiOps &ops,
                           void *ws, size_t stride, void *res, const PeerArgs &pa) {
-    vexb::reduce_multi_kernel<T, 4><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
+    if (vexb::expr_has_temps(e)) vexb::reduce_multi_kernel<T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
+    else                         vexb::reduce_multi_kernel<T, 4, false><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
 }
 
 extern "C" int vexb_reduce_multi(int dev, void *stream, const vexb_expr *expr, int dtype, size_t n, size_t index_offset,
