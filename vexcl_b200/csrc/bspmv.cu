@@ -464,29 +464,18 @@ static std::string usr_source(const vexb_usr_ops &o, size_t val_bytes) {
     return s.str();
 }
 
-// Compiled kernels by (snippets, val_bytes, device): the front ends pass the same ops on every call, and this key is much
-// shorter than the source jit_build would otherwise compare.
-static std::mutex g_usr_mx;
-static std::map<std::pair<std::string, int>, void *> g_usr_fns;
-
-// The device's program header goes first in the source (the snippets may use what it declares) and into the key.
+// One kernel per (snippets, val_bytes): the front ends pass the same ops on every call.  The device's program header goes
+// first in the source (the snippets may use what it declares).
 static int usr_kernel(int dev, const vexb_usr_ops &o, size_t val_bytes, void **fn) {
-    const std::string header = program_header(dev);
-    std::string key;
-    for (const char *part : {o.val_type, o.rhs_type, o.decl, o.product, o.append, header.c_str()}) {
+    std::string key = "usr:";
+    for (const char *part : {o.val_type, o.rhs_type, o.decl, o.product, o.append}) {
         key += std::to_string(strlen(part)); key += ':'; key += part;
     }
     key += std::to_string(o.rhs_bytes) + ":" + std::to_string(val_bytes);
-    const auto k = std::make_pair(key, dev);
-    {
-        std::lock_guard<std::mutex> lock(g_usr_mx);
-        auto it = g_usr_fns.find(k);
-        if (it != g_usr_fns.end()) { *fn = it->second; return VEXB_OK; }
-    }
-    VEXB_TRY(jit_build(dev, with_program_header(header, usr_source(o, val_bytes)), "vexb_usr_kernel", fn));
-    std::lock_guard<std::mutex> lock(g_usr_mx);
-    g_usr_fns[k] = *fn;
-    return VEXB_OK;
+    return jit_program(dev, key, "vexb_usr_kernel", program_header(dev), [&](JitBuild *b) {
+        b->text = usr_source(o, val_bytes);
+        return VEXB_OK;
+    }, true, fn);
 }
 
 } // namespace vexb
@@ -559,17 +548,5 @@ extern "C" int vexb_jit_source_usr(const vexb_usr_ops *ops, int val_bytes, char 
     VEXB_CHECK(len, "len is NULL");
     VEXB_TRY(usr_check_ops(ops));
     VEXB_CHECK(val_bytes >= 1 && val_bytes <= 64 && val_bytes % 4 == 0, "val_bytes %d is not a multiple of 4 in 4..64", val_bytes);
-    std::string src = usr_source(*ops, (size_t)val_bytes);
-    if (compile) {
-        size_t cubin = 0; std::string log;
-        VEXB_TRY(jit_compile_only(src, &cubin, &log));
-        src += "// NVRTC: ok, cubin " + std::to_string(cubin) + " bytes\n";
-        if (!log.empty()) src += "/* log:\n" + log + "*/\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return jit_print(usr_source(*ops, (size_t)val_bytes), compile, false, buf, len);
 }

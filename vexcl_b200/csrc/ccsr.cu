@@ -294,7 +294,8 @@ static int launch_jit(vexb_ccsr *A, cudaStream_t st, const T *x, T *y, T alpha, 
     if (A->jit_failed || A->m > CCSR_JIT_MAX_ROWS || A->nnz > CCSR_JIT_MAX_NNZ) return VEXB_OK;
     if (!A->jit_fn) {
         const std::string src = ccsr_jit_source(A->val_dtype, A->idx_bytes, A->hrow, A->hcol, A->hval);
-        if (jit_build(A->dev, src, "vexb_ccsr_jit", &A->jit_fn) != VEXB_OK) { A->jit_failed = true; return VEXB_OK; }   // generic kernel instead
+        if (jit_program(A->dev, "ccsr:" + src, "vexb_ccsr_jit", std::string(), [&](JitBuild *b) { b->text = src; return VEXB_OK; }, true,
+                        &A->jit_fn) != VEXB_OK) { A->jit_failed = true; return VEXB_OK; }   // generic kernel instead
     }
     unsigned long long n = A->n;
     const void *idx = A->idx;
@@ -458,16 +459,5 @@ extern "C" int vexb_ccsr_jit_source(size_t m, const int32_t *row, const int32_t 
     std::vector<int> hrow(row, row + m + 1), hcol(col, col + row[m]);
     std::vector<double> hval((size_t)row[m]);
     for (int j = 0; j < row[m]; ++j) hval[(size_t)j] = val_dtype == VEXB_F64 ? ((const double *)val)[j] : (double)((const float *)val)[j];
-    std::string src = ccsr_jit_source(val_dtype, idx_bytes, hrow, hcol, hval);
-    if (compile) {
-        size_t bytes = 0; std::string log;
-        VEXB_TRY(jit_compile_only(src, &bytes, &log));
-        src += "// NVRTC: ok, cubin " + std::to_string(bytes) + " bytes\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return jit_print(ccsr_jit_source(val_dtype, idx_bytes, hrow, hcol, hval), compile, false, buf, len);
 }

@@ -3,9 +3,10 @@
 // For those -- and, opt-in through the tunable "eval.jit", for any expression that has no hand-written
 // sweep -- the IR is printed as CUDA C (one statement per IR instruction), compiled ONCE with NVRTC for
 // sm_90a (--fmad=false, so results stay bit-identical to the interpreter and the unfused CPU loop),
-// cached by source text, and launched through the driver API on the caller's stream.  This is the only
-// place where the build resembles the reference's run-time code generation (vexcl/operations.hpp:1841-1884,
-// vexcl/backend/cuda/compiler.hpp:53-115); it needs libnvrtc and libcuda at run time, both dlopen()ed.
+// kept in the program cache that every run-time kernel shares (jit_program), and launched through the
+// driver API on the caller's stream.  This is the only place where the build resembles the reference's
+// run-time code generation (vexcl/operations.hpp:1841-1884, vexcl/backend/cuda/compiler.hpp:53-115); it
+// needs libnvrtc and libcuda at run time, both dlopen()ed.
 #include "exprhost.hpp"
 #include "jit.hpp"
 #include "spmat.hpp"
@@ -46,7 +47,8 @@ std::string program_header(int dev) {
     return it == g_headers.end() || it->second.empty() ? std::string() : it->second.back();
 }
 
-std::string with_program_header(const std::string &header, const std::string &src) {
+// `src` with `header` at its very top (on a line of its own); `src` itself when the header is empty.
+static std::string with_program_header(const std::string &header, const std::string &src) {
     if (header.empty()) return src;
     return header + (header.back() == '\n' ? "" : "\n") + src;
 }
@@ -755,7 +757,7 @@ static std::atomic<bool> g_bg_cancel{false};       // set while the process is l
 constexpr int VEXB_ERR_CANCELLED = -100;           // internal only, never returned through the ABI
 
 // device_default: --device-as-default-execution-space, for programs with a preamble (program_has_preamble) only.
-static int compile_cubin(const std::string &src, std::vector<char> *cubin, std::string *log, bool device_default = false) {
+static int compile_cubin(const std::string &src, std::vector<char> *cubin, std::string *log, bool device_default) {
     VEXB_TRY(load_nvrtc());
     std::lock_guard<std::mutex> nvrtc_lock(g_nvrtc_mx);
     if (g_bg_cancel.load()) return VEXB_ERR_CANCELLED;                 // queued behind another compilation while the process exits
@@ -840,13 +842,13 @@ static int check_ccsr_terms(const vexb_expr &e, int dev, const void *lhs, size_t
     return VEXB_OK;
 }
 
-// One cache entry per request shape.  state: 0 new, 1 compiling (a thread owns it), 2 cubin ready, 3 failed.
+// One cache entry per program.  state: 0 new, 1 compiling (a thread owns it), 2 cubin ready, 3 failed.
 struct JitEntry {
     std::mutex mx; std::condition_variable cv;
     int state = 0; long uses = 0;
-    int status = VEXB_OK; std::string error;           // of a failed compilation (reported to synchronous callers)
+    int status = VEXB_OK; std::string error;           // of a failed compilation (returned to every later request)
     std::vector<char> cubin;
-    std::map<int, CUfunction> fn;                       // per device, loaded by the first caller on that device
+    std::map<int, CUfunction> fn;                       // per device, loaded by the first request on that device
 };
 static std::map<std::string, std::shared_ptr<JitEntry>> g_entries;
 
@@ -873,35 +875,96 @@ struct BackgroundJoinGuard {
 };
 static thread_local BackgroundJoinGuard tl_bg_guard;
 
-// NVRTC front to back for one entry; runs WITHOUT the global lock (hundreds of milliseconds), on the caller's thread
-// (mode 1) or on a background thread (mode 2).
-// header: the device's program header when the request was made (header_for), "" for none.
-static void compile_entry(std::shared_ptr<JitEntry> en, std::vector<vexb_expr> es, int lhs_dtype, int aop, std::string header) {
-    std::string src, err;
+// NVRTC for one entry; runs WITHOUT any lock of the cache (hundreds of milliseconds), on the requesting thread or on a
+// background thread.
+static void compile_entry(std::shared_ptr<JitEntry> en, std::string src, bool device_default) {
     std::vector<char> cubin;
-    std::vector<const vexb_expr *> ps;
-    for (const vexb_expr &x : es) ps.push_back(&x);
-    int st = generate_source_n(ps.data(), (int)ps.size(), lhs_dtype, aop, &src);
-    if (st == VEXB_OK) st = compile_cubin(with_program_header(header, src), &cubin, nullptr, program_has_preamble(ps.data(), (int)ps.size()));
-    if (st == VEXB_ERR_CANCELLED) {                                     // the process is leaving: back to "never tried"
-        std::lock_guard<std::mutex> lock(en->mx);
-        en->state = 0;
-        en->cv.notify_all();
-        return;
-    }
-    if (st != VEXB_OK) err = vexb_last_error();
+    const int st = compile_cubin(src, &cubin, nullptr, device_default);
+    const std::string err = st == VEXB_OK ? std::string() : std::string(vexb_last_error());
     std::lock_guard<std::mutex> lock(en->mx);
-    if (st == VEXB_OK) { en->cubin.swap(cubin); en->state = 2; }
+    if (st == VEXB_ERR_CANCELLED) en->state = 0;                       // the process is leaving: back to "never tried"
+    else if (st == VEXB_OK) { en->cubin.swap(cubin); en->state = 2; }
     else { en->status = st; en->error = err; en->state = 3; }
     en->cv.notify_all();
 }
 
-static void spawn_background(std::shared_ptr<JitEntry> en, const std::vector<vexb_expr> &e, int lhs_dtype, int aop, const std::string &header) {
+static void spawn_background(std::shared_ptr<JitEntry> en, std::string src, bool device_default) {
     std::lock_guard<std::mutex> bl(g_bg_mx);
     static bool registered = false;
     if (!registered) { registered = true; atexit(join_background_compilations); }
-    g_bg_threads.emplace_back(compile_entry, en, e, lhs_dtype, aop, header);
+    g_bg_threads.emplace_back(compile_entry, en, std::move(src), device_default);
     tl_bg_guard.armed = true;
+}
+
+int jit_program(int dev, const std::string &key, const char *name, const std::string &header, const JitSource &source,
+                bool wait, void **fn) {
+    *fn = nullptr;
+    std::shared_ptr<JitEntry> en;
+    {
+        std::lock_guard<std::mutex> lock(g_jmx);                      // short: map lookup only
+        auto &slot = g_entries[key_with_header(key, header)];
+        if (!slot) slot = std::make_shared<JitEntry>();
+        en = slot;
+    }
+    std::unique_lock<std::mutex> lock(en->mx);
+    if (en->state == 0) {
+        JitBuild b;
+        b.uses = ++en->uses;
+        const int st = source(&b);
+        if (st != VEXB_OK) { en->state = 3; en->status = st; en->error = vexb_last_error(); }
+        else if (b.later) return VEXB_OK;
+        else {
+            en->state = 1;
+            std::string src = with_program_header(header, b.text);
+            if (b.background) { spawn_background(en, std::move(src), b.device_default); return VEXB_OK; }
+            lock.unlock();
+            compile_entry(en, std::move(src), b.device_default);
+            lock.lock();
+        }
+    }
+    if (en->state == 1) {
+        if (!wait) return VEXB_OK;
+        en->cv.wait(lock, [&] { return en->state != 1; });
+    }
+    if (en->state == 3) { set_error(__FILE__, __LINE__, "%s", en->error.c_str()); return en->status; }
+    if (en->state != 2) VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "the compilation of %s was cancelled: the process is exiting", name);
+    if (dev < 0) return VEXB_OK;
+    auto it = en->fn.find(dev);
+    if (it == en->fn.end()) {
+        VEXB_TRY(load_driver());
+        VEXB_CUDA(cudaFree(0));                                       // make sure the primary context is current
+        CUmodule mod = nullptr;
+        CUfunction f = nullptr;
+        const char *what = "cuModuleLoadData";
+        CUresult r = g_jit.cuModuleLoadData(&mod, en->cubin.data());
+        if (r == 0) { what = "cuModuleGetFunction"; r = g_jit.cuModuleGetFunction(&f, mod, name); }
+        if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "%s(%s) failed: %s", what, name, m); }
+        it = en->fn.emplace(dev, f).first;
+    }
+    *fn = it->second;
+    return VEXB_OK;
+}
+
+int jit_launch(void *fn, unsigned grid, unsigned block, unsigned smem, cudaStream_t st, void **args) {
+    CUresult r = g_jit.cuLaunchKernel((CUfunction)fn, grid, 1, 1, block, 1, 1, smem, (CUstream)st, args, nullptr);
+    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuLaunchKernel failed: %s", m); }
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return VEXB_OK;
+}
+
+int jit_print(std::string src, int compile, bool device_default, char *buf, size_t *len) {
+    if (compile) {
+        std::vector<char> cubin; std::string log;
+        VEXB_TRY(compile_cubin(src, &cubin, &log, device_default));
+        src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
+        if (!log.empty()) src += "/* log:\n" + log + "*/\n";
+    }
+    if (buf) {
+        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
+        memcpy(buf, src.c_str(), src.size() + 1);
+    }
+    *len = src.size() + 1;
+    return VEXB_OK;
 }
 
 // mode 1: the specialised kernel is mandatory (user functions, eval.jit = 1): compile now if nobody has, wait if somebody
@@ -909,7 +972,8 @@ static void spawn_background(std::shared_ptr<JitEntry> en, const std::vector<vex
 // an NVRTC compilation on a background thread and returns at once; the pre-compiled interpreter serves this and the next
 // launches (no start-up stall) until the cubin is ready, then every launch takes the specialised kernel.  Both produce the
 // same bits, so the switch is invisible.  `eval.jit_after` (0) delays the compilation until a shape has been used that
-// often.  *done = false means "not handled here" (the caller runs the interpreter).
+// often, `eval.jit_sync` (0) compiles on the requesting thread instead.  *done = false means "not handled here" (the
+// caller runs the interpreter).
 int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const vexb_expr &e, size_t n, size_t index_offset,
              int mode, bool *done) {
     *done = false;
@@ -917,55 +981,15 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     VEXB_TRY(sell_sweep_term(e, &sell));                              // before the cache: the signature does not tell strips apart
     VEXB_TRY(check_ccsr_terms(e, dev, lhs, n, index_offset));
     const vexb_expr *pe = &e;
-    const std::string header = header_for(dev, &pe, 1);
-    std::shared_ptr<JitEntry> en;
-    {
-        std::lock_guard<std::mutex> lock(g_jmx);                      // short: map lookup only
-        auto &slot = g_entries[key_with_header(request_signature(e, lhs_dtype, aop), header)];
-        if (!slot) slot = std::make_shared<JitEntry>();
-        en = slot;
-    }
-    CUfunction fn = nullptr;
-    {
-        std::unique_lock<std::mutex> lock(en->mx);
-        ++en->uses;
-        if (en->state == 0) {
-            if (mode == 2 && en->uses <= param("eval.jit_after", 0)) return VEXB_OK;
-            int s0 = load_driver();
-            if (s0 == VEXB_OK) s0 = load_nvrtc();
-            if (s0 != VEXB_OK) { en->state = 3; en->status = s0; en->error = vexb_last_error(); }
-            else {
-                en->state = 1;
-                if (mode == 2 && !param("eval.jit_sync", 0)) {
-                    spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop, header);
-                    return VEXB_OK;                                    // the interpreter serves meanwhile
-                }
-                lock.unlock();
-                compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, aop, header);
-                lock.lock();
-            }
-        }
-        if (en->state == 1) {
-            if (mode == 2) return VEXB_OK;                            // still compiling: interpreter
-            en->cv.wait(lock, [&] { return en->state != 1; });
-        }
-        if (en->state == 3) {
-            if (mode == 2) return VEXB_OK;
-            set_error(__FILE__, __LINE__, "%s", en->error.c_str());
-            return en->status;
-        }
-        auto it = en->fn.find(dev);
-        if (it != en->fn.end()) fn = it->second;
-        else {
-            VEXB_CUDA(cudaFree(0));                                   // make sure the primary context is current
-            CUmodule mod = nullptr;
-            CUresult r = g_jit.cuModuleLoadData(&mod, en->cubin.data());
-            if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleLoadData failed: %s", m); }
-            r = g_jit.cuModuleGetFunction(&fn, mod, "vexb_jit_kernel");
-            if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleGetFunction failed: %s", m); }
-            en->fn[dev] = fn;
-        }
-    }
+    void *fn = nullptr;
+    const int s = jit_program(dev, request_signature(e, lhs_dtype, aop), "vexb_jit_kernel", header_for(dev, &pe, 1), [&](JitBuild *b) -> int {
+        if (mode == 2 && b->uses <= param("eval.jit_after", 0)) { b->later = true; return VEXB_OK; }
+        b->background = mode == 2 && !param("eval.jit_sync", 0);
+        b->device_default = program_has_preamble(&pe, 1);
+        return generate_source(e, lhs_dtype, aop, &b->text);
+    }, mode != 2, &fn);
+    if (mode == 2 && !fn) return VEXB_OK;                             // not ready, or failed: the interpreter serves
+    VEXB_TRY(s);
     *done = true;
     terms_host tt;
     VEXB_TRY(pack_terms(e, dev, n, &tt));
@@ -978,16 +1002,12 @@ int jit_eval(int dev, cudaStream_t st, void *lhs, int lhs_dtype, int aop, const 
     const size_t cap = (size_t)sm_count(dev) * 64;
     if (blocks > cap) blocks = cap;
     if (sell >= 0) blocks = (static_cast<const vexb_spmat *>(e.term[sell].v.ptr)->n_slices + 7) / 8;   // a thread per stored lane, no loop
-    CUresult r = g_jit.cuLaunchKernel(fn, (unsigned)blocks, 1, 1, 256, 1, 1, 0, (CUstream)st, args, nullptr);
-    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuLaunchKernel failed: %s", m); }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return VEXB_OK;
+    return jit_launch(fn, (unsigned)blocks, 256, 0, st, args);
 }
 
-// The components of a multi-expression assignment in one kernel (generate_source_n).  Same modes as jit_eval; *done =
-// false means "not served here" (NVRTC missing, still compiling in the background, more than 8 components, a sparse
-// product among the terminals): the caller evaluates component by component.
-struct multi_host { terms_host c[8]; void *lhs[8]; };
+// The components of a multi-expression assignment in one kernel (generate_source_n).  Same modes as jit_eval, without
+// eval.jit_after; *done = false means "not served here" (NVRTC missing or failed, still compiling in the background, more
+// than 8 components, a sparse product among the terminals): the caller evaluates component by component.
 int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lhs_dtype, int aop, const vexb_expr *const *es,
                    size_t n, size_t index_offset, int mode, bool *done) {
     *done = false;
@@ -1003,54 +1023,18 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
         key += "temps:";
         for (int c = 0; c < ncomp; ++c) for (int k = 0; k < VEXB_MAX_TEMPS; ++k) key.push_back((char)tc.cls[c][k]);
     }
-    const std::string header = header_for(dev, es, ncomp);
-    std::shared_ptr<JitEntry> en;
-    {
-        std::lock_guard<std::mutex> lock(g_jmx);
-        auto &slot = g_entries[key_with_header("multi:" + key, header)];
-        if (!slot) slot = std::make_shared<JitEntry>();
-        en = slot;
-    }
-    CUfunction fn = nullptr;
-    {
-        std::unique_lock<std::mutex> lock(en->mx);
-        ++en->uses;
-        if (en->state == 0) {
-            int s0 = load_driver();
-            if (s0 == VEXB_OK) s0 = load_nvrtc();
-            if (s0 != VEXB_OK) { en->state = 3; en->status = s0; en->error = vexb_last_error(); }
-            else {
-                en->state = 1;
-                std::vector<vexb_expr> copy;
-                for (int c = 0; c < ncomp; ++c) copy.push_back(*es[c]);
-                if (mode == 2 && !param("eval.jit_sync", 0)) { spawn_background(en, copy, lhs_dtype, aop, header); return VEXB_OK; }
-                lock.unlock();
-                compile_entry(en, copy, lhs_dtype, aop, header);
-                lock.lock();
-            }
-        }
-        if (en->state == 1) {
-            if (mode == 2) return VEXB_OK;
-            en->cv.wait(lock, [&] { return en->state != 1; });
-        }
-        if (en->state != 2) return VEXB_OK;                           // failed or cancelled: component by component
-        auto it = en->fn.find(dev);
-        if (it != en->fn.end()) fn = it->second;
-        else {
-            VEXB_CUDA(cudaFree(0));
-            CUmodule mod = nullptr;
-            CUresult r = g_jit.cuModuleLoadData(&mod, en->cubin.data());
-            if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleLoadData failed: %s", m); }
-            r = g_jit.cuModuleGetFunction(&fn, mod, "vexb_jit_kernel");
-            if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleGetFunction failed: %s", m); }
-            en->fn[dev] = fn;
-        }
-    }
+    void *fn = nullptr;
+    jit_program(dev, "multi:" + key, "vexb_jit_kernel", header_for(dev, es, ncomp), [&](JitBuild *b) {
+        b->background = mode == 2 && !param("eval.jit_sync", 0);
+        b->device_default = program_has_preamble(es, ncomp);
+        return generate_source_n(es, ncomp, lhs_dtype, aop, &b->text);
+    }, mode != 2, &fn);
+    if (!fn) return VEXB_OK;
     // kernel parameter: struct multi_j { terms_j c[ncomp]; T *lhs[ncomp]; } -- packed for the actual ncomp
     std::vector<unsigned char> prm((size_t)ncomp * sizeof(terms_host) + (size_t)ncomp * sizeof(void *), 0);
     for (int c = 0; c < ncomp; ++c) {
-        terms_host tt; memset(&tt, 0, sizeof(tt));
-        for (int k = 0; k < es[c]->n_terms; ++k) tt.t[k] = es[c]->term[k];
+        terms_host tt;
+        VEXB_TRY(pack_terms(*es[c], dev, n, &tt));
         memcpy(prm.data() + (size_t)c * sizeof(terms_host), &tt, sizeof(tt));
         memcpy(prm.data() + (size_t)ncomp * sizeof(terms_host) + (size_t)c * sizeof(void *), &lhs[c], sizeof(void *));
     }
@@ -1059,9 +1043,7 @@ int jit_eval_multi(int dev, cudaStream_t st, int ncomp, void *const *lhs, int lh
     size_t blocks = (n + 255) / 256;
     const size_t cap = (size_t)sm_count(dev) * 32;
     if (blocks > cap) blocks = cap;
-    CUresult r = g_jit.cuLaunchKernel(fn, (unsigned)blocks, 1, 1, 256, 1, 1, 0, (CUstream)st, args, nullptr);
-    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuLaunchKernel failed: %s", m); }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    VEXB_TRY(jit_launch(fn, (unsigned)blocks, 256, 0, st, args));
     *done = true;
     return VEXB_OK;
 }
@@ -1074,74 +1056,23 @@ int jit_pending() {
     return 0;
 }
 
-// ---- helpers for other run-time specialised kernels (jit.hpp) ---------------------------------------------------------
-int jit_compile_only(const std::string &src, size_t *cubin_bytes, std::string *log, bool device_default) {
-    std::vector<char> cubin;
-    VEXB_TRY(compile_cubin(src, &cubin, log, device_default));
-    if (cubin_bytes) *cubin_bytes = cubin.size();
-    return VEXB_OK;
-}
-
-// Kernels built from complete source text (CCSR row code, stencil operators): keyed by the text itself, per device.
-static std::map<std::pair<std::string, int>, CUfunction> g_built;
-static std::mutex g_bmx;
-
-int jit_build(int dev, const std::string &src, const char *name, void **fn, bool device_default) {
-    const std::pair<std::string, int> key(src + "\n//" + name + (device_default ? "\n//device-as-default-execution-space" : ""), dev);
-    std::lock_guard<std::mutex> lock(g_bmx);                          // builds are rare and serialised; launches do not come here
-    auto it = g_built.find(key);
-    if (it != g_built.end()) { *fn = it->second; return VEXB_OK; }
-    VEXB_TRY(load_driver());
-    std::vector<char> cubin;
-    VEXB_TRY(compile_cubin(src, &cubin, nullptr, device_default));
-    VEXB_CUDA(cudaFree(0));                                           // make sure the primary context is current
-    CUmodule mod = nullptr;
-    CUfunction f = nullptr;
-    CUresult r = g_jit.cuModuleLoadData(&mod, cubin.data());
-    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleLoadData failed: %s", m); }
-    r = g_jit.cuModuleGetFunction(&f, mod, name);
-    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuModuleGetFunction(%s) failed: %s", name, m); }
-    g_built[key] = f;
-    *fn = f;
-    return VEXB_OK;
-}
-
-int jit_launch(void *fn, unsigned grid, unsigned block, unsigned smem, cudaStream_t st, void **args) {
-    CUresult r = g_jit.cuLaunchKernel((CUfunction)fn, grid, 1, 1, block, 1, 1, smem, (CUstream)st, args, nullptr);
-    if (r != 0) { const char *m = ""; g_jit.cuGetErrorString(r, &m); VEXB_FAIL(VEXB_ERR_CUDA, "cuLaunchKernel failed: %s", m); }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    return VEXB_OK;
-}
-
 // One launch per slot for a reduction of an expression with user functions or inlined sparse products (see
 // generate_reduce_source).  Compiled synchronously at its first use, then cached per request shape, dtype, ops and
 // skeleton, and per device.  VEXB_ERR_UNSUPPORTED only when NVRTC cannot be loaded: the front ends then evaluate the
 // expression into a temporary and reduce that.  The caller has selected `dev` and handled n == 0.
 int jit_reduce(int dev, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t index_offset, int nops, const int *ops,
                bool multi, size_t cap, void *d_result, void *d_workspace, const PeerArgs &pa) {
-    static std::mutex mx;
-    static std::map<std::pair<std::string, int>, void *> fns;
     VEXB_TRY(check_ccsr_terms(e, dev, nullptr, n, index_offset));
     const int skel = reduce_skeleton(e, dtype, multi);
     const vexb_expr *pe = &e;
-    const std::string header = header_for(dev, &pe, 1);
     std::string key = "reduce:" + request_signature(e, host_result_type(e), VEXB_SET);
     key.push_back('|'); key.push_back((char)dtype); key.push_back((char)skel); key.push_back((char)nops);
     for (int k = 0; k < nops; ++k) key.push_back((char)ops[k]);
-    key = key_with_header(key, header);
     void *fn = nullptr;
-    {
-        std::lock_guard<std::mutex> lock(mx);
-        auto it = fns.find(std::make_pair(key, dev));
-        if (it != fns.end()) fn = it->second;
-    }
-    if (!fn) {
-        std::string src;
-        VEXB_TRY(generate_reduce_source(e, dtype, nops, ops, skel, &src));
-        VEXB_TRY(jit_build(dev, with_program_header(header, src), "vexb_reduce_kernel", &fn, program_has_preamble(&pe, 1)));
-        std::lock_guard<std::mutex> lock(mx);
-        fns[std::make_pair(key, dev)] = fn;
-    }
+    VEXB_TRY(jit_program(dev, key, "vexb_reduce_kernel", header_for(dev, &pe, 1), [&](JitBuild *b) {
+        b->device_default = program_has_preamble(&pe, 1);
+        return generate_reduce_source(e, dtype, nops, ops, skel, &b->text);
+    }, true, &fn));
     terms_host tt;
     VEXB_TRY(pack_terms(e, dev, n, &tt));
     size_t blocks;
@@ -1209,25 +1140,13 @@ extern "C" int vexb_jit_precompile(int lhs_dtype, int assign_op, const vexb_expr
     VEXB_TRY(normalize_expr(expr, &e, false));
     int sell = -1;
     VEXB_TRY(sell_sweep_term(e, &sell));
-    VEXB_TRY(load_nvrtc());
-    std::shared_ptr<JitEntry> en;
-    {
-        std::lock_guard<std::mutex> lock(g_jmx);
-        auto &slot = g_entries[request_signature(e, lhs_dtype, assign_op)];
-        if (!slot) slot = std::make_shared<JitEntry>();
-        en = slot;
-    }
-    std::unique_lock<std::mutex> lock(en->mx);
-    if (en->state == 0) {
-        en->state = 1;
-        if (background) { spawn_background(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op, std::string()); return VEXB_OK; }
-        lock.unlock();
-        compile_entry(en, std::vector<vexb_expr>(1, e), lhs_dtype, assign_op, std::string());
-        lock.lock();
-    }
-    if (!background && en->state == 1) en->cv.wait(lock, [&] { return en->state != 1; });
-    if (en->state == 3) { set_error(__FILE__, __LINE__, "%s", en->error.c_str()); return en->status; }
-    return VEXB_OK;
+    void *fn = nullptr;
+    const vexb_expr *pe = &e;
+    return jit_program(-1, request_signature(e, lhs_dtype, assign_op), "vexb_jit_kernel", std::string(), [&](JitBuild *b) {
+        b->background = background != 0;
+        b->device_default = program_has_preamble(&pe, 1);
+        return generate_source(e, lhs_dtype, assign_op, &b->text);
+    }, !background, &fn);
 }
 
 extern "C" int vexb_jit_pending(int *pending) {
@@ -1293,18 +1212,7 @@ extern "C" int vexb_jit_source_multi_dev(int dev, int lhs_dtype, int assign_op, 
     }
     std::string src;
     VEXB_TRY(generate_source_n(ps.data(), ncomp, lhs_dtype, assign_op, &src));
-    src = with_program_header(header_for(dev, ps.data(), ncomp), src);
-    if (compile) {
-        std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(ps.data(), ncomp)));
-        src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return jit_print(with_program_header(header_for(dev, ps.data(), ncomp), src), compile, program_has_preamble(ps.data(), ncomp), buf, len);
 }
 
 extern "C" int vexb_jit_source(int lhs_dtype, int assign_op, const vexb_expr *expr, char *buf, size_t *len, int compile) {
@@ -1321,19 +1229,7 @@ extern "C" int vexb_jit_source_dev(int dev, int lhs_dtype, int assign_op, const 
     std::string src;
     VEXB_TRY(generate_source(e, lhs_dtype, assign_op, &src));
     const vexb_expr *pe = &e;
-    src = with_program_header(header_for(dev, &pe, 1), src);
-    if (compile) {
-        std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(&pe, 1)));
-        src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
-        if (!log.empty()) src += "/* log:\n" + log + "*/\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return jit_print(with_program_header(header_for(dev, &pe, 1), src), compile, program_has_preamble(&pe, 1), buf, len);
 }
 
 // The kernel vexb_reduce_all (nops == 1) or vexb_reduce_multi (nops > 1) generates for a reduction of this expression in
@@ -1360,17 +1256,5 @@ extern "C" int vexb_jit_source_reduce_dev(int dev, int dtype, int nops, const in
     std::string src;
     VEXB_TRY(generate_reduce_source(e, dtype, nops, mo, reduce_skeleton(e, dtype, nops > 1), &src));
     const vexb_expr *pe = &e;
-    src = with_program_header(header_for(dev, &pe, 1), src);
-    if (compile) {
-        std::vector<char> cubin; std::string log;
-        VEXB_TRY(compile_cubin(src, &cubin, &log, program_has_preamble(&pe, 1)));
-        src += "// NVRTC: ok, cubin " + std::to_string(cubin.size()) + " bytes\n";
-        if (!log.empty()) src += "/* log:\n" + log + "*/\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return jit_print(with_program_header(header_for(dev, &pe, 1), src), compile, program_has_preamble(&pe, 1), buf, len);
 }

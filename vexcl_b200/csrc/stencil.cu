@@ -374,17 +374,7 @@ extern "C" int vexb_stencil_operator_source(int id, char *buf, size_t *len, int 
         VEXB_CHECK(id >= 0 && (size_t)id < vexb::g_sops.size(), "unknown stencil operator %d", id);
         src = vexb::stencil_op_source(vexb::g_sops[(size_t)id]);
     }
-    if (compile) {
-        size_t bytes = 0; std::string log;
-        VEXB_TRY(vexb::jit_compile_only(src, &bytes, &log));
-        src += "// NVRTC: ok, cubin " + std::to_string(bytes) + " bytes\n";
-    }
-    if (buf) {
-        VEXB_CHECK(*len > src.size(), "buffer too small (%zu <= %zu)", *len, src.size());
-        memcpy(buf, src.c_str(), src.size() + 1);
-    }
-    *len = src.size() + 1;
-    return VEXB_OK;
+    return vexb::jit_print(std::move(src), compile, false, buf, len);
 }
 
 extern "C" int vexb_stencil_operator_apply(int dev, void *stream, int id, const void *x, size_t n, const void *left,
@@ -400,8 +390,11 @@ extern "C" int vexb_stencil_operator_apply(int dev, void *stream, int id, const 
     VEXB_CHECK(n < ((size_t)1 << 38), "slice too long");
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     void *fn = nullptr;
-    // the operator's body is user text: the device's program header goes first, and is part of the cache key (the text)
-    VEXB_TRY(vexb::jit_build(dev, vexb::with_program_header(vexb::program_header(dev), vexb::stencil_op_source(op)), "vexb_stencil_op", &fn));
+    // the operator's body is user text: the device's program header goes first
+    VEXB_TRY(vexb::jit_program(dev, "stencil:" + std::to_string(id), "vexb_stencil_op", vexb::program_header(dev), [&](vexb::JitBuild *b) {
+        b->text = vexb::stencil_op_source(op);
+        return VEXB_OK;
+    }, true, &fn));
     long long nn = (long long)n;
     double a64 = alpha; float a32 = (float)alpha;
     void *args[] = {&x, &nn, &left, &right, &y, op.dtype == VEXB_F64 ? (void *)&a64 : (void *)&a32, &append};
