@@ -116,7 +116,7 @@ typedef enum {
                              spmat/inline_spmv.hpp:68-76).  Expressions with such terminals run on the NVRTC side path
                              (the row loop is generated into the kernel, specialised to the strip's format and width),
                              reductions of them included (vexb_reduce_all / vexb_reduce_multi). */
-    VEXB_TERM_CCSR = 5    /* v.ptr: a vexb_ccsr (host handle); pad[0]: slot of the VEXB_TERM_VEC holding x; pad[1]: the
+    VEXB_TERM_CCSR = 5,   /* v.ptr: a vexb_ccsr (host handle); pad[0]: slot of the VEXB_TERM_VEC holding x; pad[1]: the
                              matrix's idx width on the device (vexb_ccsr_info.idx_bytes: 1, 2 or 4); dtype: the matrix's
                              value type, which is also x's.  Element i evaluates to
                                  s = 0;  s = s + val[j] * x[i + col[j]]  for j over the unique row idx[i], in storage order,
@@ -131,7 +131,25 @@ typedef enum {
                              pad[0] names a vector terminal of that type, pad[1] agrees with the handle.  vexb_eval returns
                              VEXB_ERR_UNSUPPORTED when x is the assignment's target (threads would write x[i] while others
                              read x[i + col[j]]): evaluate the product into a temporary first. */
+    VEXB_TERM_PTR = 6     /* v.ptr: the device address of element 0 of an array of `dtype` (vex::raw_pointer,
+                             vexcl/vector_pointer.hpp); pad[0..5]: the array's element count, little-endian.  It gives the
+                             expression no size.  An element is read by VEXB_OP_LOAD, and a LOAD outside [0, count) reads 0
+                             without touching memory: every branch of a SELECT is evaluated, so `i > 0 ? p[i - 1] : 0` must
+                             not fault at i = 0, as the reference's lazy `?:` does not.  A VEXB_OP_TERM on it
+                             pushes the pointer itself, with type VEXB_PTR(dtype), which is legal only as the argument of a
+                             VEXB_OP_CALL whose function declared that parameter VEXB_PTR(dtype).  Pointers travel in the
+                             terminal table as vectors do, so one compiled kernel serves every pointer of one request shape.
+                             NULL is refused outside the source printers.  vexb_eval and vexb_eval_multi return
+                             VEXB_ERR_UNSUPPORTED, before any launch, when a pointer addresses a target slice (threads would read
+                             elements that others overwrite): the front ends then redirect it to a device copy of the vector.
+                             vexb_eval_multi reports no "not handled" fall-back in that case, since component by component
+                             would race too.  Pointers are not taken by stencil operators or as a sparse product's x. */
 } vexb_term_kind;
+
+/* The type of a pointer to `dtype` elements: the value a VEXB_OP_TERM on a VEXB_TERM_PTR pushes, and a parameter type of
+ * vexb_function_register(_ex) (never a return type).  A function registered with VEXB_F64 and one with VEXB_PTR(VEXB_F64)
+ * for the same parameter are two functions. */
+#define VEXB_PTR(dtype) ((dtype) | 0x10)
 
 typedef struct {
     uint8_t kind;   /* vexb_term_kind */
@@ -182,13 +200,25 @@ typedef enum {
      * dtype and pointer or value) is computed once per element by the generated kernel and handed to both. */
     VEXB_OP_TDEF,
     VEXB_OP_TREF,
+    /* Subscript and dereference through a raw pointer (the reference grammar's `a[b]` and `*p`, operations.hpp:493-494):
+     * `arg` is the slot of a VEXB_TERM_PTR terminal and `type` is its dtype; pops one VEXB_I64 index and pushes ptr[index],
+     * or 0 when the index is outside [0, count) of the terminal.
+     * The front ends fold C pointer arithmetic into the index: each offset is widened on its own (signed types
+     * sign-extended, unsigned zero-extended, U64 reinterpreted), then the offsets are added in I64, so *(p + a), *(p - a),
+     * p[a], (p + a)[b], a + p and *p are all one LOAD.  Refused with VEXB_ERR_INVALID by every entry point, before any
+     * launch or NVRTC run: an `arg` that is not a pointer terminal, an index that is not I64, a `type` other than the
+     * pointer's dtype, and a pointer value anywhere but a matching call parameter (arithmetic, CVT, TDEF, SELECT, the
+     * result).  vexb_eval and the reductions serve such programs with the interpreter or the generated kernel, never a
+     * hand-written sweep.  Loads take the read-only path in generated kernels unless the kernel passes a pointer to a
+     * user function, whose body may write through it. */
+    VEXB_OP_LOAD,
     VEXB_OP_COUNT_
 } vexb_opcode;
 
 typedef struct {
     uint8_t  op;    /* vexb_opcode */
     uint8_t  type;  /* vexb_dtype  */
-    uint16_t arg;   /* TERM: term slot; CVT: source dtype; CALL: function id; TDEF / TREF: temporary slot */
+    uint16_t arg;   /* TERM / LOAD: term slot; CVT: source dtype; CALL: function id; TDEF / TREF: temporary slot */
 } vexb_instr;
 
 typedef struct {
@@ -267,7 +297,8 @@ int vexb_partition(size_t n, int nparts, const double *weights, size_t *part);
 int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int assign_op,
               const vexb_expr *expr, size_t n, size_t index_offset);
 /* User-defined device functions (VEX_FUNCTION, vexcl/function.hpp:225): `body` is C source that refers to its
- * arguments as prm1, prm2, ... (the reference's convention) and returns a value of `ret_dtype`.
+ * arguments as prm1, prm2, ... (the reference's convention) and returns a value of `ret_dtype`.  An argument type may
+ * be VEXB_PTR(dtype): the parameter is then `T *prmK`, and the call passes a VEXB_TERM_PTR terminal.
  * Such functions cannot be pre-compiled: an expression that calls one is turned into CUDA source
  * (the sweep skeleton with the expression inlined), compiled once with NVRTC for sm_90a, cached, and launched
  * through the driver API.  Setting the tunable "eval.jit" = 1 sends every non-sweep expression down the same
@@ -344,6 +375,8 @@ int vexb_eval_path(int lhs_dtype, int assign_op, const vexb_expr *expr, char *bu
  * kernel NVRTC generates for the request (compiled at its first use, then cached): the row loop or the call feeds the
  * fold directly, and the result has the bits of evaluating the expression into a vector of its own type and reducing
  * that vector with the same tunables.  VEXB_ERR_UNSUPPORTED when NVRTC cannot be loaded: reduce such a temporary then.
+ * Expressions that load through raw pointers (VEXB_OP_LOAD) are reduced by such a kernel too, unless "eval.jit" is 0;
+ * then, and when NVRTC cannot be loaded, by the interpreter.
  * ---------------------------------------------------------------------- */
 typedef struct vexb_peer vexb_peer;   /* a group of GPUs that write each other's memory; see "Peer memory" below */
 int vexb_reduce_workspace_bytes(int dev, size_t *bytes);

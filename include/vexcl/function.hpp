@@ -86,9 +86,24 @@ VEXCL_BUILTIN_3(fma, VEXB_OP_FMA, true)     VEXCL_BUILTIN_3(mad, VEXB_OP_FMA, tr
 // ---- user-defined functions ------------------------------------------------------------------------
 namespace detail {
 
+/// The IR type of an argument spelled `t`.  `T*` and `const T*` over the six element types are pointer parameters
+/// (VEXB_PTR(T)), which take a vex::raw_pointer (vector_pointer.hpp).
 inline int dtype_from_name(std::string t) {
     std::string u;
     for (char c : t) if (!std::isspace(static_cast<unsigned char>(c))) u += c;
+    if (!u.empty() && u.back() == '*') {
+        std::string e = u.substr(0, u.size() - 1);
+        if (e.compare(0, 5, "const") == 0) e = e.substr(5);
+        if (e.compare(0, 3, "cl_") == 0) e = e.substr(3);
+        // only the six element types: bool, char and short would name arrays of another element size
+        if (e == "double") return VEXB_PTR(VEXB_F64);
+        if (e == "float") return VEXB_PTR(VEXB_F32);
+        if (e == "int") return VEXB_PTR(VEXB_I32);
+        if (e == "uint" || e == "unsigned" || e == "unsignedint") return VEXB_PTR(VEXB_U32);
+        if (e == "long" || e == "longlong" || e == "ptrdiff_t") return VEXB_PTR(VEXB_I64);
+        if (e == "ulong" || e == "size_t" || e == "unsignedlong" || e == "unsignedlonglong") return VEXB_PTR(VEXB_U64);
+        throw std::runtime_error("VEX_FUNCTION: unsupported pointer argument type '" + t + "'");
+    }
     if (u.compare(0, 3, "cl_") == 0) u = u.substr(3);
     if (u == "double") return VEXB_F64;
     if (u == "float") return VEXB_F32;
@@ -111,14 +126,21 @@ inline void parse_arguments(const std::string &seq, std::vector<int> &types, std
         std::string type = seq.substr(pos + 1, comma - pos - 1), name = seq.substr(comma + 1, end - comma - 1);
         name.erase(0, name.find_first_not_of(" \t")); name.erase(name.find_last_not_of(" \t") + 1);
         types.push_back(dtype_from_name(type));
+        if (types.back() & VEXB_PTR(0)) {             // T *name = prmK; (const T *name for a const T* parameter)
+            const bool c = type.find("const") != std::string::npos;
+            prologue += std::string(c ? "const " : "") + dtype_c_name(types.back() & ~VEXB_PTR(0)) + " *" + name + " = prm" + std::to_string(types.size()) + "; ";
+        } else
         prologue += std::string("const ") + dtype_c_name(types.back()) + " " + name + " = prm" + std::to_string(types.size()) + "; ";
         pos = end + 1;
     }
 }
+/// The IR type of a parameter of a signature: T* and const T* are pointer parameters (VEXB_PTR).
+template <class A> struct param_dtype { static const int value = dtype_of<typename promoted<A>::type>::value; };
+template <class A> struct param_dtype<A*> { static const int value = VEXB_PTR(dtype_of<typename std::remove_cv<A>::type>::value); };
 template <class T> struct signature_types;
 template <class R, class... A> struct signature_types<R(A...)> {
     typedef R result;
-    static std::vector<int> args() { return std::vector<int>{dtype_of<typename promoted<A>::type>::value...}; }
+    static std::vector<int> args() { return std::vector<int>{param_dtype<A>::value...}; }
 };
 
 } // namespace detail
@@ -139,10 +161,16 @@ struct call_node : vector_expr_tag {
     void props(detail::expr_props &p) const { props_args(p, std::index_sequence_for<Args...>()); }
     private:
         template <size_t... I> void lower_args(detail::ir_builder &b, std::index_sequence<I...>) const {
-            int dummy[] = {0, (b.cvt(std::get<I>(args).lower(b), arg_types[I]), 0)...}; (void)dummy;
+            int dummy[] = {0, (arg(b, std::get<I>(args).lower(b), arg_types[I]), 0)...}; (void)dummy;
         }
         template <size_t... I> void props_args(detail::expr_props &p, std::index_sequence<I...>) const {
             int dummy[] = {0, (std::get<I>(args).props(p), 0)...}; (void)dummy;
+        }
+        // a pointer parameter takes a raw_pointer of its element type, and a raw_pointer goes to nothing else
+        static void arg(detail::ir_builder &b, int t, int declared) {
+            precondition(!((t | declared) & VEXB_PTR(0)) || t == declared,
+                         "user function: a T* parameter takes a vex::raw_pointer of a vector<T>, and a raw_pointer goes to nothing else");
+            b.cvt(t, declared);
         }
 };
 

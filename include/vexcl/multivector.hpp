@@ -104,14 +104,27 @@ void assign_components(const std::array<vex::vector<T>*, N> &lhs, const Rhs &rhs
     // One generated kernel for all components (vexb_eval_multi): reads of element i all happen before its writes, so no
     // temporaries whatever reads what.  Served once the kernel for this tuple of expressions exists (it is compiled in
     // the background at first use); until then -- and for anything it does not take -- component by component below.
+    std::vector<backend::device_vector<T>> copies(N * nd);          // [device][target]: what raw pointers into a target read
     {
         bool fused = N >= 2 && N <= 8;
         for (unsigned d = 0; d < nd && fused; ++d) {
             const void *es[N]; void *out[N];
             for (size_t i = 0; i < N; ++i) { es[i] = &ir[i * nd + d].e; out[i] = (*lhs[i])(d).raw(); }
             int handled = 0;
-            VEXB_CHECKED(vexb_eval_multi(queue[d].ordinal(), queue[d].raw(), (int)N, out, dtype_of<T>::value, OP::op,
-                                         reinterpret_cast<const vexb_expr *const *>(es), lhs[0]->part_size(d), lhs[0]->part_start(d), &handled));
+            int st = vexb_eval_multi(queue[d].ordinal(), queue[d].raw(), (int)N, out, dtype_of<T>::value, OP::op,
+                                     reinterpret_cast<const vexb_expr *const *>(es), lhs[0]->part_size(d), lhs[0]->part_start(d), &handled);
+            // raw pointers into a target read a device copy of it instead (never component by component: that would race
+            // too); the component-by-component path below stages through temporaries, so it reads the old targets as is
+            bool redirected = false;
+            if (st == VEXB_ERR_UNSUPPORTED)
+                for (size_t j = 0; j < N; ++j)
+                    for (size_t i = 0; i < N; ++i)
+                        redirected = redirect_pointers(ir[i * nd + d].e, out[j], dtype_of<T>::value, lhs[j]->part_size(d) * sizeof(T), queue[d],
+                                                       copies[d * N + j]) || redirected;
+            if (redirected)
+                st = vexb_eval_multi(queue[d].ordinal(), queue[d].raw(), (int)N, out, dtype_of<T>::value, OP::op,
+                                     reinterpret_cast<const vexb_expr *const *>(es), lhs[0]->part_size(d), lhs[0]->part_start(d), &handled);
+            VEXB_CHECKED(st);
             if (!handled) {
                 // all devices or none: a kernel that is ready is ready for every device, so only d == 0 can say no
                 fused = false;

@@ -10,7 +10,8 @@
  *
  * Accepted operators = the reference grammar's (operations.hpp:457-506):
  *   + - * / %   unary + -   < > <= >= == !=   && || !   & | ^ << >>
- * plus builtin functions (function.hpp), if_else, element_index, tagged terminals.
+ * plus builtin functions (function.hpp), if_else, element_index, tagged terminals, and the subscript and
+ * dereference of a vex::raw_pointer (vector_pointer.hpp).
  * Arithmetic scalars are by-value terminals (operations.hpp:168-175).  Node value
  * types follow C++'s usual arithmetic conversions; comparisons and logical operators
  * yield int.
@@ -102,6 +103,15 @@ struct ir_builder {
         emit(VEXB_OP_TERM, dtype, k);
     }
     void cvt(int from, int to) { if (from != to) emit(VEXB_OP_CVT, to, from); }
+    /// A raw pointer (VEXB_TERM_PTR): the device address of element 0 of an array of `count` elements of `dtype` (a load
+    /// outside them reads 0).  Returns its slot, for a VEXB_OP_LOAD or a VEXB_OP_TERM that passes the pointer to a user
+    /// function.
+    int ptr_term(const void *ptr, int dtype, size_t count) {
+        int k = new_term();
+        e.term[k].kind = VEXB_TERM_PTR; e.term[k].dtype = static_cast<uint8_t>(dtype); e.term[k].v.ptr = ptr;
+        for (int b = 0; b < 6; ++b) e.term[k].pad[b] = static_cast<uint8_t>(static_cast<unsigned long long>(count) >> (8 * b));
+        return k;
+    }
 
     // ---- temporaries (vex::make_temp, temporary.hpp) ----
     // The program is code[0, n_prefix), the definitions in post-order (each ends with its VEXB_OP_TDEF), then the
@@ -139,7 +149,7 @@ struct ir_builder {
             for (int pc = from; pc < to; ++pc) {
                 const vexb_instr &in = e.code[pc];
                 d.append(reinterpret_cast<const char*>(&in), sizeof(in) - sizeof(in.arg));
-                if (in.op != VEXB_OP_TERM) { d.append(reinterpret_cast<const char*>(&in.arg), sizeof(in.arg)); continue; }
+                if (in.op != VEXB_OP_TERM && in.op != VEXB_OP_LOAD) { d.append(reinterpret_cast<const char*>(&in.arg), sizeof(in.arg)); continue; }
                 vexb_term t = e.term[in.arg];
                 const bool product = t.kind == VEXB_TERM_SPMV || t.kind == VEXB_TERM_CCSR;
                 if (product) t.pad[0] = 0;
@@ -173,6 +183,15 @@ struct expr_props {
     void see(const std::vector<backend::command_queue> &q, const std::vector<size_t> &p, size_t n) {
         if (!queue) { queue = &q; part = p; }
         see_size(n);
+        see_devices(q);
+    }
+    /// A raw pointer (vector_pointer.hpp): its queue list, but no size or partition (expression_properties of the
+    /// reference's vector_pointer).  Every vector of such an expression must have one part, on the pointer's device.
+    void see_pointer(const std::vector<backend::command_queue> &q) {
+        if (!queue) queue = &q;
+        precondition(ptr_dev < 0 || ptr_dev == q[0].ordinal(), "raw pointers of one expression must live on one device");
+        ptr_dev = q[0].ordinal();
+        see_devices(q);
     }
     void see_size(size_t n) {
         if (!sized) { size = n; sized = true; }
@@ -180,6 +199,17 @@ struct expr_props {
     }
     size_t part_size(unsigned d) const { return part.empty() ? 0 : part[d + 1] - part[d]; }
     size_t part_start(unsigned d) const { return part.empty() ? 0 : part[d]; }
+    private:
+        int ptr_dev = -1;           ///< device of the expression's raw pointers, -1 without
+        bool several_parts = false; ///< some vector of the expression has more than one part
+        std::vector<int> devs;      ///< devices of the one-part vectors
+        void see_devices(const std::vector<backend::command_queue> &q) {
+            if (q.size() != 1) several_parts = true;
+            else devs.push_back(q[0].ordinal());
+            if (ptr_dev < 0) return;
+            precondition(!several_parts, "raw_pointer: every vector of the expression must have one part");
+            for (int d : devs) precondition(d == ptr_dev, "raw_pointer: every vector of the expression must live on the pointer's device");
+        }
 };
 
 template <class T> struct promoted {
@@ -563,6 +593,26 @@ operator-(const mixed_expression<E, T> &m, const X &x) {
 
 namespace detail {
 
+/// Point the raw-pointer terminals of `e` that address `target` at a device copy of it (`copy`: made here unless it holds
+/// one already; the caller keeps it until the launch is enqueued, and freeing waits for the device).  The back end refuses a pointer into the
+/// target (VEXB_ERR_UNSUPPORTED): threads would read elements that others overwrite.  Through the copy, `x = p[(i + 1) %
+/// n]` with p = raw_pointer(x) rotates x and every element reads the old values.  False when no terminal addresses it.
+template <class T>
+bool redirect_pointers(vexb_expr &e, const void *target, int dtype, size_t bytes, const backend::command_queue &q,
+                       backend::device_vector<T> &copy) {
+    bool hit = false;
+    for (int k = 0; k < e.n_terms; ++k) hit = hit || (e.term[k].kind == VEXB_TERM_PTR && e.term[k].v.ptr == target);
+    if (!hit) return false;
+    precondition(bytes % sizeof(T) == 0, "raw_pointer: bad target size");
+    if (!copy.raw()) {
+        copy = backend::device_vector<T>(q, bytes / sizeof(T));
+        if (bytes) VEXB_CHECKED(vexb_d2d(q.ordinal(), copy.raw(), target, bytes, q.raw()));
+    }
+    for (int k = 0; k < e.n_terms; ++k)
+        if (e.term[k].kind == VEXB_TERM_PTR && e.term[k].v.ptr == target && e.term[k].dtype == dtype) e.term[k].v.ptr = copy.raw();
+    return true;
+}
+
 /// lhs OP= expr on every device slice (replaces assign_expression, operations.hpp:1818-1897).
 template <class OP, class T, class Expr>
 void assign_expression(vex::vector<T> &lhs, const Expr &expr, int comp = -1) {
@@ -576,8 +626,13 @@ void assign_expression(vex::vector<T> &lhs, const Expr &expr, int comp = -1) {
     for (unsigned d = 0; d < queue.size(); ++d) {
         ir_builder b(d, comp);
         expr.lower(b);
-        VEXB_CHECKED(vexb_eval(queue[d].ordinal(), queue[d].raw(), lhs(d).raw(), dtype_of<T>::value, OP::op,
-                               &b.e, lhs.part_size(d), lhs.part_start(d)));
+        int st = vexb_eval(queue[d].ordinal(), queue[d].raw(), lhs(d).raw(), dtype_of<T>::value, OP::op,
+                           &b.e, lhs.part_size(d), lhs.part_start(d));
+        backend::device_vector<T> copy;
+        if (st == VEXB_ERR_UNSUPPORTED && redirect_pointers(b.e, lhs(d).raw(), dtype_of<T>::value, lhs.part_size(d) * sizeof(T), queue[d], copy))
+            st = vexb_eval(queue[d].ordinal(), queue[d].raw(), lhs(d).raw(), dtype_of<T>::value, OP::op,
+                           &b.e, lhs.part_size(d), lhs.part_start(d));
+        VEXB_CHECKED(st);
     }
 }
 

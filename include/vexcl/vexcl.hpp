@@ -16,6 +16,7 @@
 #include "constants.hpp"
 #include "tagged_terminal.hpp"
 #include "temporary.hpp"
+#include "vector_pointer.hpp"
 #include "reductor.hpp"
 #include "spmat.hpp"
 #include "spmat/ccsr.hpp"

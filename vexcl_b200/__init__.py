@@ -11,7 +11,8 @@ from ._lib import (F64, F32, I32, U32, I64, U64, SET, ADD, SUB, MUL, DIV, MOD, A
 from .api import (Context, vector, Reductor, SpMat, SpMatCCSR, BlockMatrix, ComplexMatrix, UserValueMatrix, stencil, partition, ElementIndex, Scalar, if_else,
                   sin, cos, tan, asin, acos, atan, sinh, cosh, tanh, exp, exp2, log, log2, log10, sqrt, rsqrt,
                   cbrt, fabs, floor, ceil, round_, trunc, pow_, atan2, fmod, hypot, fmin, fmax, fma, make_inline, InlineSpMV, assign_multi,
-                  UserFunction, push_program_header, pop_program_header, program_header, make_temp, Temp)
+                  UserFunction, push_program_header, pop_program_header, program_header, make_temp, Temp,
+                  raw_pointer, deref, ptr, Pointer, Load)
 
 
 def set_param(name: str, value: int):

@@ -16,14 +16,20 @@ ERR_CUDA, ERR_INVALID, ERR_NCCL, ERR_UNSUPPORTED, ERR_NOMEM, ERR_PEER = range(1,
 F64, F32, I32, U32, I64, U64 = range(6)
 SET, ADD, SUB, MUL, DIV, MOD, AND, OR, XOR, LSH, RSH = range(11)
 SUM, SUM_KAHAN, MAX, MIN, MINMAX = range(5)
-TERM_VEC, TERM_SCALAR, TERM_INDEX, TERM_DSCALAR, TERM_SPMV, TERM_CCSR = range(6)
+TERM_VEC, TERM_SCALAR, TERM_INDEX, TERM_DSCALAR, TERM_SPMV, TERM_CCSR, TERM_PTR = range(7)
 FMT_AUTO, FMT_CSR, FMT_HELL, FMT_PATTERNS, FMT_SELL = range(5)
 FMT_VALUES_F32 = 0x100          # ORed into fmt: double values stored as float, double vectors and sums
 MAX_TERMS, MAX_CODE, MAX_STACK, MAX_TEMPS = 16, 64, 12, 8
 
+
+def PTR(dtype: int) -> int:
+    """VEXB_PTR(dtype): the type of a pointer to `dtype` elements (a user function's pointer parameter)."""
+    return dtype | 0x10
+
+
 _OPS = ("TERM CVT NEG LNOT ADD SUB MUL DIV MOD BAND BOR BXOR SHL SHR LT GT LE GE EQ NE LAND LOR SELECT "
         "SIN COS TAN ASIN ACOS ATAN SINH COSH TANH EXP EXP2 LOG LOG2 LOG10 SQRT RSQRT CBRT FABS FLOOR CEIL "
-        "ROUND TRUNC POW ATAN2 FMOD HYPOT FMIN FMAX FMA CALL TDEF TREF").split()
+        "ROUND TRUNC POW ATAN2 FMOD HYPOT FMIN FMAX FMA CALL TDEF TREF LOAD").split()
 OP = {name: i for i, name in enumerate(_OPS)}
 
 

@@ -292,25 +292,39 @@ def if_else(cond, a, b): return Select(cond, a, b)
 
 
 class Call(Node):
-    """Call of a user-defined device function (VEX_FUNCTION)."""
+    """Call of a user-defined device function (VEX_FUNCTION).  A raw_pointer goes to a parameter declared ptr(dtype)."""
     def __init__(self, fn: "UserFunction", args):
-        self.fn, self.args = fn, [wrap(a) for a in args]
+        self.fn, self.args = fn, [a if isinstance(a, Pointer) else wrap(a) for a in args]
+        for a, t in zip(self.args, fn.arg_types):
+            if isinstance(a, Pointer) and (a.offsets or t != L.PTR(a.dtype)):
+                raise TypeError(f"{fn.name}: a raw_pointer without arithmetic goes to a parameter declared ptr() of its type")
+            if not isinstance(a, Pointer) and t & 0x10:
+                raise TypeError(f"{fn.name}: a ptr() parameter takes a raw_pointer")
         self.dtype = fn.ret
+
+
+class ptr:
+    """The type of a pointer parameter of a UserFunction: ptr(np.float64) is `double *`, ptr(np.float64, const=True)
+    `const double *` (the same parameter to the library: the constness only goes into the prologue)."""
+    def __init__(self, dtype, const: bool = False):
+        self.dtype, self.const = _vdt(dtype), bool(const)
 
 
 class UserFunction:
     """VEX_FUNCTION(ret, name, (type, arg)..., body) (vexcl/function.hpp:225): a device function given as C source.
-    `args` is a list of (numpy dtype, name); inside `body` the arguments are available under their names (and, as in
-    the reference's older form, as prm1, prm2, ...).  Expressions that call it run on the NVRTC side path.
+    `args` is a list of (numpy dtype or ptr(dtype), name); inside `body` the arguments are available under their names
+    (and, as in the reference's older form, as prm1, prm2, ...).  Expressions that call it run on the NVRTC side path.
     deps: UserFunctions the body calls by their names (VEX_FUNCTION_D); every program that calls this one holds them.
     preamble: file-scope text (helpers, macros) before the definition (VEX_FUNCTION_V1_WITH_PREAMBLE); helpers in it
     need no __device__."""
 
     def __init__(self, ret, name: str, args, body: str, deps=(), preamble: str = ""):
         self.ret = _vdt(ret)
-        self.arg_types = [_vdt(t) for t, _ in args]
+        self.arg_types = [L.PTR(t.dtype) if isinstance(t, ptr) else _vdt(t) for t, _ in args]
         ctypes_names = {L.F64: "double", L.F32: "float", L.I32: "int", L.U32: "unsigned int", L.I64: "long long", L.U64: "unsigned long long"}
-        prologue = "".join(f"const {ctypes_names[t]} {nm} = prm{k + 1}; " for k, (t, (_, nm)) in enumerate(zip(self.arg_types, args)))
+        prologue = "".join((f"{'const ' if t.const else ''}{ctypes_names[t.dtype]} *{nm} = prm{k + 1}; " if isinstance(t, ptr)
+                            else f"const {ctypes_names[at]} {nm} = prm{k + 1}; ")
+                           for k, (at, (t, nm)) in enumerate(zip(self.arg_types, args)))
         fid = C.c_int(-1)
         at = (C.c_int * max(len(args), 1))(*self.arg_types)
         dep_ids = [d.id if isinstance(d, UserFunction) else int(d) for d in deps]
@@ -340,6 +354,60 @@ class Temp(Node):
 def make_temp(tag: int, expr, dtype=None) -> Temp:
     """vex::make_temp<tag>(expr), or vex::make_temp<tag, dtype>(expr)."""
     return Temp(tag, expr, dtype)
+
+
+class Pointer:
+    """vex::raw_pointer(x) (vexcl/vector_pointer.hpp): the device address of x's element 0, for expressions that reach any
+    element.  p[i], deref(p + i), (p + a)[b], i + p and p - i read one element (VEXB_OP_LOAD: every offset is widened to
+    int64 on its own, as C does, then added; a read outside x gives 0, so a load under an if_else guard is safe); a
+    UserFunction takes p itself for a ptr() parameter.  Nothing else is
+    defined on a pointer.  x must have one slice, and every vector of an expression that holds p must live on p's
+    device."""
+    __array_ufunc__ = None
+
+    def __init__(self, vec, offsets=()):
+        self.vec, self.offsets, self.dtype = vec, tuple(offsets), vec.dtype      # offsets: (sign, node) in order
+
+    def _offset(self, o, sign):
+        if isinstance(o, Pointer):
+            raise TypeError("two pointers do not combine")
+        o = wrap(o)
+        if _is_float(o.dtype):
+            raise TypeError("pointer arithmetic takes an integral offset")
+        return Pointer(self.vec, self.offsets + ((sign, o),))
+
+    def __add__(self, o): return self._offset(o, +1)
+    def __radd__(self, o): return self._offset(o, +1)
+    def __sub__(self, o): return self._offset(o, -1)
+    def __getitem__(self, i): return Load(self._offset(i, +1))
+
+    def _refuse(self, *_):
+        raise TypeError("a raw_pointer is only indexed, offset by an integer, dereferenced or passed to a user function")
+    __rsub__ = __mul__ = __rmul__ = __truediv__ = __rtruediv__ = __mod__ = __neg__ = __lt__ = __gt__ = __le__ = __ge__ = _refuse
+    __and__ = __or__ = __xor__ = __lshift__ = __rshift__ = _refuse
+
+
+class Load(Node):
+    """One element read through a pointer: *(p + offsets).  `args` holds the offset nodes (for the tree walkers)."""
+    def __init__(self, p: Pointer):
+        self.p, self.dtype = p, p.dtype
+        self.args = [o for _, o in p.offsets]
+
+
+def raw_pointer(x) -> Pointer:
+    """vex::raw_pointer(x): refused, like the reference, for vectors of more than one slice."""
+    if not isinstance(x, vector):
+        raise TypeError("raw_pointer takes a vector")
+    if x.ctx.nparts != 1:
+        raise ValueError("raw_pointer is not supported for multi-device contexts")
+    return Pointer(x)
+
+
+def deref(p) -> Load:
+    """*p: the element p points to."""
+    if not isinstance(p, Pointer):
+        raise TypeError("deref takes a raw_pointer or pointer arithmetic on one")
+    return Load(p)
 
 
 def _header_devices(ctx: Context):
@@ -383,6 +451,8 @@ pow_, atan2, fmod, hypot, fmin, fmax, fma = (_mkfunc(o) for o in ("POW", "ATAN2"
 def wrap(x) -> Node:
     if isinstance(x, Node):
         return x
+    if isinstance(x, Pointer):
+        raise TypeError("a raw_pointer is only indexed, offset by an integer, dereferenced or passed to a user function")
     if isinstance(x, SpMVTerm) and isinstance(x.A, SpMatCCSR) and isinstance(x.x, vector):
         return CcsrProduct(x.A, x.x, x.scale)                  # a CCSR product where an operand goes
     return Scalar(x)
@@ -405,6 +475,32 @@ class _Lowering:
         # (tag, dtype, definition by content, node)
         self.n_prefix = 0
         self.temps = []
+        # raw pointers: the device they live on, and the vectors seen (each must have one slice on that device)
+        self.ptr_dev = None
+        self.vec_seen = []
+
+    def see(self, v=None, ptr_vec=None):
+        """Record a vector (or the vector behind a pointer) of the expression, and refuse a pointer next to a vector of
+        several slices or of another device, before anything is launched."""
+        if v is not None:
+            self.vec_seen.append(v)
+        if ptr_vec is not None:
+            d = ptr_vec.ctx.devs[ptr_vec.ctx.local[0]]
+            if self.ptr_dev is not None and self.ptr_dev != d:
+                raise ValueError("raw pointers of one expression must live on one device")
+            self.ptr_dev = d
+        if self.ptr_dev is not None:
+            for w in self.vec_seen:
+                if w.ctx.nparts != 1 or w.ctx.devs[w.ctx.local[0]] != self.ptr_dev:
+                    raise ValueError("every vector of an expression with a raw_pointer must have one slice, on the pointer's device")
+
+    def pointer(self, p: Pointer) -> int:
+        """The pointer's terminal: its address, and its element count in pad[0..5] (a load outside reads 0)."""
+        self.see(ptr_vec=p.vec)
+        k = self.term(L.TERM_PTR, p.dtype, ptr=p.vec.bufs[p.vec.ctx.local[0]].value or 0)
+        for b in range(6):
+            self.e.term[k].pad[b] = (p.vec.n >> (8 * b)) & 0xff
+        return k
 
     def term(self, kind, dtype, pad0: int = 0, **kw) -> int:
         k = self.e.n_terms
@@ -436,7 +532,20 @@ class _Lowering:
                 self.size, self.ctx = n.n, n.ctx
             elif n.n != self.size:
                 raise ValueError("vectors of different sizes in one expression")     # VEXCL_CHECK_SIZES, operations.hpp:1824-1840
+            self.see(n)
             self.emit("TERM", n.dtype, self.term(L.TERM_VEC, n.dtype, ptr=n.bufs[self.part].value or 0))
+        elif isinstance(n, Load):
+            # the index: every offset widened to int64 on its own (signed types sign-extended, unsigned zero-extended),
+            # then added; *p reads element 0
+            if not n.p.offsets:
+                self.lower(Scalar(0, L.I64))
+            for j, (sign, o) in enumerate(n.p.offsets):
+                self.lower(o); self.cvt(o.dtype, L.I64)
+                if j:
+                    self.emit("ADD" if sign > 0 else "SUB", L.I64)
+                elif sign < 0:
+                    self.emit("NEG", L.I64)
+            self.emit("LOAD", n.dtype, self.pointer(n.p))
         elif isinstance(n, InlineSpMV):
             if self.size is None:
                 self.size, self.ctx = n.A.n, n.A.ctx
@@ -486,6 +595,9 @@ class _Lowering:
             self.emit(n.op, n.ctype)
         elif isinstance(n, Call):
             for a, t in zip(n.args, n.fn.arg_types):
+                if isinstance(a, Pointer):
+                    self.emit("TERM", L.PTR(a.dtype), self.pointer(a))       # the pointer itself (Call checked the type)
+                    continue
                 self.lower(a); self.cvt(a.dtype, t)
             self.emit("CALL", n.fn.ret, n.fn.id)
         elif isinstance(n, Temp):
@@ -541,7 +653,7 @@ class _Lowering:
         for pc in range(frm, to):
             c = self.e.code[pc]
             out.append(bytes((c.op, c.type)))
-            if c.op != L.OP["TERM"]:
+            if c.op not in (L.OP["TERM"], L.OP["LOAD"]):
                 out.append(c.arg.to_bytes(2, "little"))
                 continue
             t = self.e.term[c.arg]
@@ -732,6 +844,8 @@ class Mixed:
 
 
 def _node_add_mixed(self, o):
+    if isinstance(o, Pointer):
+        return o + self                                # i + p: pointer arithmetic, as in C
     return Mixed.of(self) + o if isinstance(o, (SpMVTerm, Mixed)) else Node._bin(self, "ADD", o)
 
 
@@ -844,9 +958,16 @@ class vector(Node):
             low.size = self.n
             low.target = self
             low.sweep = None if sweep else False
+            low.see(self)
             low.lower(rhs)
-            L.check(lib.vexb_eval(self.ctx.devs[k], self.ctx.streams[k], self.bufs[k], self.dtype, op,
-                                  C.byref(low.e), self.part_size(k), self.part_start(k)))
+            code = lib.vexb_eval(self.ctx.devs[k], self.ctx.streams[k], self.bufs[k], self.dtype, op,
+                                 C.byref(low.e), self.part_size(k), self.part_start(k))
+            copies = _redirect_pointers(low.e, [self]) if code == L.ERR_UNSUPPORTED else []
+            if copies:
+                # a pointer into the target: threads would read elements others overwrite, so every read goes to a copy
+                code = lib.vexb_eval(self.ctx.devs[k], self.ctx.streams[k], self.bufs[k], self.dtype, op,
+                                     C.byref(low.e), self.part_size(k), self.part_start(k))
+            L.check(code)
         return self
 
     def _assign_mixed(self, op: int, m: Mixed):
@@ -892,6 +1013,25 @@ class vector(Node):
         buf = C.create_string_buffer(64)
         L.check(L.lib().vexb_eval_path(self.dtype, op, C.byref(low.e), buf, 64))
         return buf.value.decode()
+
+
+def _redirect_pointers(e, targets) -> list:
+    """Point every raw-pointer terminal of `e` that addresses one of `targets` at a device copy of that vector (what the
+    back end asks for with VEXB_ERR_UNSUPPORTED: `x = p[(i + 1) % n]` with p = raw_pointer(x) then reads the old x).
+    Returns the copies (to be kept until the launch is enqueued; freeing waits for the device), [] when none applies."""
+    copies = []
+    for v in targets:
+        k = v.ctx.local[0]
+        addr = v.bufs[k].value
+        hits = [j for j in range(e.n_terms) if e.term[j].kind == L.TERM_PTR and e.term[j].v.ptr == addr]
+        if not hits:
+            continue
+        cp = vector(v.ctx, v.n, v.np_dtype)
+        L.check(L.lib().vexb_d2d(v.ctx.devs[k], cp.bufs[k], v.bufs[k], v.part_size(k) * v.np_dtype.itemsize, v.ctx.streams[k]))
+        for j in hits:
+            e.term[j].v.ptr = cp.bufs[k].value
+        copies.append(cp)
+    return copies
 
 
 def _reduce_all_in_step(ctx, k, peer, dtype, kind, result, code, results):
@@ -1679,12 +1819,21 @@ def assign_multi(lhs, rhs, op: int = L.SET) -> bool:
         for r in rhs:
             low = _Lowering(k, lhs[0].part_start(k))
             low.size = n
+            for v in lhs:
+                low.see(v)
             low.lower(r)
             lows.append(low)
         es = (C.POINTER(L.Expr) * N)(*[C.pointer(low.e) for low in lows])
         out = (C.c_void_p * N)(*[v.bufs[k] for v in lhs])
         handled = C.c_int(0)
-        L.check(lib.vexb_eval_multi(ctx.devs[k], ctx.streams[k], N, out, dt, op, es, lhs[0].part_size(k), lhs[0].part_start(k), C.byref(handled)))
+        code = lib.vexb_eval_multi(ctx.devs[k], ctx.streams[k], N, out, dt, op, es, lhs[0].part_size(k), lhs[0].part_start(k), C.byref(handled))
+        if code == L.ERR_UNSUPPORTED:
+            # raw pointers into the targets read device copies instead (never component by component: that would race too)
+            # (the component-by-component path below evaluates into temporaries first, so it reads the old targets as is)
+            copies = [cp for low in lows for cp in _redirect_pointers(low.e, lhs)]
+            if copies:
+                code = lib.vexb_eval_multi(ctx.devs[k], ctx.streams[k], N, out, dt, op, es, lhs[0].part_size(k), lhs[0].part_start(k), C.byref(handled))
+        L.check(code)
         if not handled.value:
             fused = False                       # the kernel is not there yet (first slice says so): nothing has been written
     if fused:

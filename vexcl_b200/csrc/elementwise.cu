@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(256) sweep_kernel(T *lhs, SweepArgs a, size_t 
     }
 }
 
-template <int U, bool TEMPS>
+template <int U, bool EXT>
 __global__ void __launch_bounds__(256) interp_kernel(const __grid_constant__ vexb_expr e, void *lhs, int lhs_dtype,
                                                       size_t n, size_t index_offset) {
     const int rt = program_result_type(e);
@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) interp_kernel(const __grid_constant__ vex
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int k = 0; k < U; ++k) { idx[k] = base + (size_t)k * blockDim.x + threadIdx.x; active[k] = idx[k] < n; }
-        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
+        eval_expr<U, EXT>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int k = 0; k < U; ++k)
             if (active[k]) store_as(lhs, idx[k], convert(out[k], rt, lhs_dtype), lhs_dtype);
@@ -147,6 +147,16 @@ static bool plan_sweep(const void *lhs, int lhs_dtype, int aop, const vexb_expr 
     return true;
 }
 
+// A raw pointer that addresses a target slice: threads would read elements that others overwrite (the reference races
+// there).  VEXB_ERR_UNSUPPORTED before any launch; the front ends then redirect the pointer to a device copy.
+static int check_pointer_targets(const vexb_expr &e, void *const *lhs, int ncomp) {
+    for (int k = 0; k < e.n_terms; ++k)
+        for (int c = 0; c < ncomp; ++c)
+            if (e.term[k].kind == VEXB_TERM_PTR && e.term[k].v.ptr == lhs[c])
+                VEXB_FAIL(VEXB_ERR_UNSUPPORTED, "term %d: a raw pointer addresses target %d of the assignment; read a copy of that vector instead", k, c);
+    return VEXB_OK;
+}
+
 // Rewrite `lhs OP= rhs` (OP != SET) as a plain program: lhs = (L)((C)lhs OP (C)rhs),
 // C = common type of lhs and rhs, as C/C++ compound assignment does.
 static int fold_compound(const vexb_expr &e, const void *lhs, int lhs_dtype, int aop, vexb_expr *out) {
@@ -204,6 +214,7 @@ extern "C" int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int as
     VEXB_TRY(normalize_expr(expr, &e, n != 0));
     if (n == 0) return VEXB_OK;                    // empty partitions are legal (operations.hpp:1886)
     VEXB_CHECK(lhs != nullptr, "lhs is NULL");
+    VEXB_TRY(check_pointer_targets(e, &lhs, 1));
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);
     cudaStream_t st = (cudaStream_t)stream;
     const int sms = sm_count(dev);
@@ -244,7 +255,7 @@ extern "C" int vexb_eval(int dev, void *stream, void *lhs, int lhs_dtype, int as
     size_t want = (n + per_block - 1) / per_block;
     const size_t cap = (size_t)sms * (size_t)param("interp.blocks_per_sm", 4);
     const int blocks = (int)(want < cap ? want : cap);
-    if (expr_has_temps(prog)) interp_kernel<4, true><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
+    if (expr_extended(prog)) interp_kernel<4, true><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
     else                      interp_kernel<4, false><<<blocks, 256, 0, st>>>(prog, lhs, lhs_dtype, n, index_offset);
     VEXB_LAUNCHED();
     return VEXB_OK;
@@ -273,6 +284,7 @@ extern "C" int vexb_eval_multi(int dev, void *stream, int ncomp, void *const *lh
     }
     if (n == 0) { *handled = 1; return VEXB_OK; }
     for (int c = 0; c < ncomp; ++c) VEXB_CHECK(lhs[c] != nullptr, "lhs %d is NULL", c);
+    for (int c = 0; c < ncomp; ++c) VEXB_TRY(check_pointer_targets(es[(size_t)c], lhs, ncomp));   // before any fall-back
     const long jit_mode = param("eval.force_interp", 0) ? param("eval.jit", 0) : param("eval.jit", 2);
     if (!jit_mode || !param("eval.fuse_multi", 1)) return VEXB_OK;
     DeviceGuard g(dev); VEXB_CHECK(g.ok, "cannot select device %d", dev);

@@ -69,6 +69,26 @@ __device__ __forceinline__ V load_term(const vexb_term &t, size_t idx, size_t in
     return r;
 }
 
+// Element idx of the array of a VEXB_TERM_PTR terminal (VEXB_OP_LOAD), 0 outside [0, count).  The back end never lets a
+// kernel write an array it reads this way (a pointer into the target is refused), so the read-only path is safe.
+__device__ __forceinline__ V load_elem(const vexb_term &t, int dtype, long long idx) {
+    V r; r.u = 0;
+    unsigned long long count = 0;
+#pragma unroll
+    for (int b = 5; b >= 0; --b) count = count << 8 | t.pad[b];
+    if ((unsigned long long)idx >= count) return r;
+    const void *p = t.v.ptr;
+    switch (dtype) {
+        case VEXB_F64: r.f = __ldg((const double *)p + idx); break;
+        case VEXB_F32: r.f = (double)__ldg((const float *)p + idx); break;
+        case VEXB_I32: r.i = (long long)__ldg((const int *)p + idx); break;
+        case VEXB_U32: r.u = (unsigned long long)__ldg((const unsigned *)p + idx); break;
+        case VEXB_I64: r.i = __ldg((const long long *)p + idx); break;
+        default:       r.u = __ldg((const unsigned long long *)p + idx); break;
+    }
+    return r;
+}
+
 __device__ __forceinline__ V convert(V a, int from, int to) {
     if (from == to) return a;
     V r;
@@ -235,15 +255,16 @@ __host__ __device__ inline int program_result_type(const vexb_expr &e) {
 // Evaluate the program for U element indices at once (U independent lanes give
 // the memory system U loads in flight per terminal).  The top of the stack is
 // kept in registers; deeper entries spill to a small per-thread array.
-// TEMPS: the program may define temporaries (VEXB_OP_TDEF / VEXB_OP_TREF), kept in
-// a per-lane file beside the stack.  Programs without them take the TEMPS = false
-// instantiation, which is exactly the evaluator without those arms: two more arms in
-// the one switch cost the 32-bit reductions register spills they did not have.
-template <int U, bool TEMPS = false>
+// EXT: the program may use the extended opcodes -- temporaries (VEXB_OP_TDEF / VEXB_OP_TREF),
+// kept in a per-lane file beside the stack, and loads through raw pointers (VEXB_OP_LOAD).
+// Programs without them take the EXT = false instantiation, which is exactly the evaluator
+// without those arms: two more arms in the one switch cost the 32-bit reductions register
+// spills they did not have.
+template <int U, bool EXT = false>
 __device__ __forceinline__ void eval_expr(const vexb_expr &e, const size_t (&idx)[U], const bool (&active)[U],
                                           size_t index_offset, V (&out)[U]) {
     V st[VEXB_MAX_STACK][U];
-    V tmp[TEMPS ? VEXB_MAX_TEMPS : 1][U];
+    V tmp[EXT ? VEXB_MAX_TEMPS : 1][U];
     V tos[U];
     int d = 0;
 #pragma unroll
@@ -255,7 +276,7 @@ __device__ __forceinline__ void eval_expr(const vexb_expr &e, const size_t (&idx
     for (int pc = 0; pc < n_code; ++pc) {
         const vexb_instr in = e.code[pc];
         const int op = in.op, t = in.type;
-        if constexpr (TEMPS) {
+        if constexpr (EXT) {
             if (op == VEXB_OP_TDEF) {           // the host admits it at depth 1 only: the stack is empty after it
                 VEXB_LANES tmp[in.arg][k] = tos[k];
                 d = 0;
@@ -265,6 +286,11 @@ __device__ __forceinline__ void eval_expr(const vexb_expr &e, const size_t (&idx
                 if (d > 0) { VEXB_LANES st[d - 1][k] = tos[k]; }
                 VEXB_LANES tos[k] = tmp[in.arg][k];
                 ++d;
+                continue;
+            }
+            if (op == VEXB_OP_LOAD) {           // pops the I64 index, pushes the element; lanes past the end read nothing
+                const vexb_term &tm = e.term[in.arg];
+                VEXB_LANES tos[k] = active[k] ? load_elem(tm, t, tos[k].i) : V{0};
                 continue;
             }
         }

@@ -22,6 +22,7 @@ inline int op_arity(int op) {
     if (op >= VEXB_OP_POW && op <= VEXB_OP_FMAX) return 2;
     if (op == VEXB_OP_TDEF) return 1;
     if (op == VEXB_OP_TREF) return 0;
+    if (op == VEXB_OP_LOAD) return 1;
     return -1;
 }
 
@@ -92,6 +93,17 @@ inline bool expr_has_temps(const vexb_expr &e) {
     return false;
 }
 
+inline bool expr_has_load(const vexb_expr &e) {
+    for (int pc = 0; pc < e.n_code; ++pc) if (e.code[pc].op == VEXB_OP_LOAD) return true;
+    return false;
+}
+
+// Programs the interpreter serves with its extended opcodes (temporaries, loads through raw pointers): the EXT
+// instantiation of eval_expr (expr_eval.cuh).
+inline bool expr_extended(const vexb_expr &e) { return expr_has_temps(e) || expr_has_load(e); }
+
+inline bool is_ptr_type(int t) { return (t & VEXB_PTR(0)) != 0; }
+
 // Number of leading instructions that define temporaries: the program up to and including its last TDEF (0 without).
 inline int temp_prefix_length(const vexb_expr &e) {
     int n = 0;
@@ -117,9 +129,10 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     VEXB_CHECK(in->n_code >= 1 && in->n_code <= VEXB_MAX_CODE, "n_code=%d out of range", in->n_code);
     for (int k = 0; k < in->n_terms; ++k) {
         const vexb_term &t = in->term[k];
-        VEXB_CHECK(t.kind <= VEXB_TERM_CCSR, "term %d: bad kind %d", k, (int)t.kind);
+        VEXB_CHECK(t.kind <= VEXB_TERM_PTR, "term %d: bad kind %d", k, (int)t.kind);
         VEXB_CHECK(t.dtype <= VEXB_U64, "term %d: bad dtype %d", k, (int)t.dtype);
-        VEXB_CHECK(!need_ptrs || (t.kind != VEXB_TERM_VEC && t.kind != VEXB_TERM_DSCALAR) || t.v.ptr != nullptr, "term %d: NULL device pointer", k);
+        VEXB_CHECK(!need_ptrs || (t.kind != VEXB_TERM_VEC && t.kind != VEXB_TERM_DSCALAR && t.kind != VEXB_TERM_PTR) || t.v.ptr != nullptr,
+                   "term %d: NULL device pointer", k);
         if (t.kind == VEXB_TERM_SPMV) {
             VEXB_CHECK(t.v.ptr != nullptr, "term %d: NULL matrix handle", k);
             VEXB_CHECK(t.pad[0] < in->n_terms && in->term[t.pad[0]].kind == VEXB_TERM_VEC && in->term[t.pad[0]].dtype == t.dtype,
@@ -134,7 +147,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
                        "term %d: the CCSR product's x must be a vector terminal of the matrix's value type", k);
         }
     }
-    // 1. de-duplicate vector terminals (same pointer, same dtype) and drop unused ones.
+    // 1. de-duplicate vector and pointer terminals (same kind, same pointer, same dtype) and drop unused ones.
     int remap[VEXB_MAX_TERMS];
     for (int k = 0; k < VEXB_MAX_TERMS; ++k) remap[k] = -1;
     memset(out, 0, sizeof(*out));
@@ -144,6 +157,17 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     int temp_type[VEXB_MAX_TEMPS];
     for (int k = 0; k < VEXB_MAX_TEMPS; ++k) temp_type[k] = -1;
     int stype[VEXB_MAX_CODE + 1];
+    // the output slot of input terminal `k`: vectors, device scalars and pointers shared by address and type
+    auto shared_slot = [&](int k) {
+        const vexb_term &t = in->term[k];
+        int slot = remap[k];
+        if (slot < 0 && (t.kind == VEXB_TERM_VEC || t.kind == VEXB_TERM_DSCALAR || t.kind == VEXB_TERM_PTR)) {
+            for (int j = 0; j < out->n_terms; ++j)
+                if (out->term[j].kind == t.kind && out->term[j].v.ptr == t.v.ptr && out->term[j].dtype == t.dtype &&
+                    (t.kind != VEXB_TERM_PTR || memcmp(out->term[j].pad, t.pad, sizeof(t.pad)) == 0)) { slot = j; break; }
+        }
+        return slot;
+    };
     for (int pc = 0; pc < in->n_code; ++pc) {
         vexb_instr ins = in->code[pc];
         int ar = op_arity(ins.op);
@@ -153,8 +177,26 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
             VEXB_CHECK(ins.type == function_ret_dtype(ins.arg), "instr %d: call result type does not match the declaration", pc);
         }
         VEXB_CHECK(ar >= 0, "instr %d: unknown opcode %d", pc, (int)ins.op);
-        VEXB_CHECK(ins.type <= VEXB_U64, "instr %d: bad type %d", pc, (int)ins.type);
+        const bool ptr_push = ins.op == VEXB_OP_TERM && ins.arg < in->n_terms && in->term[ins.arg].kind == VEXB_TERM_PTR;
+        VEXB_CHECK(ins.type <= VEXB_U64 || (ptr_push && ins.type == VEXB_PTR(in->term[ins.arg].dtype)), "instr %d: bad type %d", pc, (int)ins.type);
         VEXB_CHECK(depth >= ar, "instr %d: stack underflow", pc);
+        // a pointer value (VEXB_OP_TERM on a VEXB_TERM_PTR) goes to a call parameter declared with its type, and nowhere else
+        for (int q = 0; q < ar; ++q) {
+            const int have = stype[depth - ar + q];
+            if (ins.op == VEXB_OP_CALL && (is_ptr_type(have) || is_ptr_type(function_arg_dtype(ins.arg, q))))
+                VEXB_CHECK(have == function_arg_dtype(ins.arg, q), "instr %d: argument %d of the call is %s, the function declares %s", pc, q,
+                           is_ptr_type(have) ? "a pointer" : "a value", is_ptr_type(function_arg_dtype(ins.arg, q)) ? "a pointer of another type" : "a value");
+            else VEXB_CHECK(ins.op == VEXB_OP_CALL || !is_ptr_type(have), "instr %d: a raw pointer is only passed to a user function (read an element with VEXB_OP_LOAD)", pc);
+        }
+        if (ins.op == VEXB_OP_LOAD) {
+            VEXB_CHECK(ins.arg < in->n_terms && in->term[ins.arg].kind == VEXB_TERM_PTR, "instr %d: LOAD reads through a pointer terminal", pc);
+            VEXB_CHECK(stype[depth - 1] == VEXB_I64, "instr %d: the index of a LOAD is I64, not type %d", pc, stype[depth - 1]);
+            VEXB_CHECK(ins.type == in->term[ins.arg].dtype, "instr %d: LOAD of type %d through a pointer of type %d", pc, (int)ins.type, (int)in->term[ins.arg].dtype);
+            int slot = shared_slot(ins.arg);
+            if (slot < 0) { VEXB_CHECK(out->n_terms < VEXB_MAX_TERMS, "too many terminals"); slot = out->n_terms++; out->term[slot] = in->term[ins.arg]; }   // pad: the count
+            remap[ins.arg] = slot;
+            ins.arg = (uint16_t)slot;
+        }
         if (ins.op == VEXB_OP_TDEF || ins.op == VEXB_OP_TREF) {
             VEXB_CHECK(ins.arg < VEXB_MAX_TEMPS, "instr %d: temporary slot %d out of range (at most %d temporaries)", pc, (int)ins.arg, VEXB_MAX_TEMPS);
             if (ins.op == VEXB_OP_TDEF) {
@@ -175,11 +217,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
         if (ins.op == VEXB_OP_TERM) {
             VEXB_CHECK(ins.arg < in->n_terms, "instr %d: term slot %d out of range", pc, (int)ins.arg);
             const vexb_term &t = in->term[ins.arg];
-            int slot = remap[ins.arg];
-            if (slot < 0 && (t.kind == VEXB_TERM_VEC || t.kind == VEXB_TERM_DSCALAR)) {
-                for (int j = 0; j < out->n_terms; ++j)
-                    if (out->term[j].kind == t.kind && out->term[j].v.ptr == t.v.ptr && out->term[j].dtype == t.dtype) { slot = j; break; }
-            }
+            int slot = shared_slot(ins.arg);
             if (slot < 0 && is_product_term(t.kind)) {
                 // the x it multiplies: an ordinary vector terminal (shared with other uses of the same vector)
                 const vexb_term &xt = in->term[t.pad[0]];
@@ -198,10 +236,10 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
                     if (t.kind == VEXB_TERM_CCSR) out->term[slot].pad[1] = t.pad[1];      // idx width
                 }
             }
-            if (slot < 0) { slot = out->n_terms++; out->term[slot] = t; memset(out->term[slot].pad, 0, sizeof(t.pad)); }
+            if (slot < 0) { slot = out->n_terms++; out->term[slot] = t; if (t.kind != VEXB_TERM_PTR) memset(out->term[slot].pad, 0, sizeof(t.pad)); }
             remap[ins.arg] = slot;
             ins.arg = (uint16_t)slot;
-            ins.type = (t.kind == VEXB_TERM_INDEX) ? VEXB_U64 : t.dtype;
+            ins.type = (t.kind == VEXB_TERM_INDEX) ? VEXB_U64 : t.kind == VEXB_TERM_PTR ? VEXB_PTR(t.dtype) : t.dtype;
         } else if (ins.op == VEXB_OP_CVT) {
             VEXB_CHECK(ins.arg <= VEXB_U64, "instr %d: bad CVT source type", pc);
             // 2. fold a conversion applied directly to a scalar terminal.
@@ -244,10 +282,12 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
         out->code[out->n_code++] = ins;
     }
     VEXB_CHECK(depth == 1, "program leaves %d values on the stack (expected 1)", depth);
+    VEXB_CHECK(!is_ptr_type(stype[0]), "the result of a program is a value, not a raw pointer");
     VEXB_CHECK(maxdepth <= VEXB_MAX_STACK, "expression too deep (%d > %d)", maxdepth, VEXB_MAX_STACK);
     // 3. compact away scalar slots orphaned by folding
     bool used[VEXB_MAX_TERMS] = {false};
-    for (int pc = 0; pc < out->n_code; ++pc) if (out->code[pc].op == VEXB_OP_TERM) used[out->code[pc].arg] = true;
+    auto names_term = [](int op) { return op == VEXB_OP_TERM || op == VEXB_OP_LOAD; };
+    for (int pc = 0; pc < out->n_code; ++pc) if (names_term(out->code[pc].op)) used[out->code[pc].arg] = true;
     for (int k = 0; k < out->n_terms; ++k) if (used[k] && is_product_term(out->term[k].kind)) used[out->term[k].pad[0]] = true;
     int newslot[VEXB_MAX_TERMS]; int n = 0;
     for (int k = 0; k < out->n_terms; ++k) newslot[k] = used[k] ? n++ : -1;
@@ -255,7 +295,7 @@ inline int normalize_expr(const vexb_expr *in, vexb_expr *out, bool need_ptrs = 
     for (int k = 0; k < out->n_terms; ++k) if (used[k] && newslot[k] != k) out->term[newslot[k]] = out->term[k];
     for (int k = n; k < out->n_terms; ++k) memset(&out->term[k], 0, sizeof(vexb_term));
     out->n_terms = n;
-    for (int pc = 0; pc < out->n_code; ++pc) if (out->code[pc].op == VEXB_OP_TERM) out->code[pc].arg = (uint16_t)newslot[out->code[pc].arg];
+    for (int pc = 0; pc < out->n_code; ++pc) if (names_term(out->code[pc].op)) out->code[pc].arg = (uint16_t)newslot[out->code[pc].arg];
     return VEXB_OK;
 }
 

@@ -69,6 +69,8 @@ static const char *ufield(int dt) {
         case VEXB_U32: return "u32"; case VEXB_I64: return "i64"; default: return "u64";
     }
 }
+// A parameter type of a user function: the value types, and `T *` for VEXB_PTR(T).
+static std::string param_ctype(int dt) { return is_ptr_type(dt) ? std::string(ctype(dt & ~VEXB_PTR(0))) + " *" : std::string(ctype(dt)); }
 static bool is_f(int t) { return t == VEXB_F64 || t == VEXB_F32; }
 static bool is_signed(int t) { return t == VEXB_I32 || t == VEXB_I64; }
 
@@ -107,7 +109,7 @@ static int emit_user_functions(const vexb_expr *const *es, int ncomp, std::ostre
         s << "__device__ __forceinline__ " << ctype(f.ret) << " " << f.name;
         if (!as_plain) s << "_" << id;
         s << "(";
-        for (size_t k = 0; k < f.args.size(); ++k) s << (k ? ", " : "") << ctype(f.args[k]) << " prm" << (k + 1);
+        for (size_t k = 0; k < f.args.size(); ++k) s << (k ? ", " : "") << param_ctype(f.args[k]) << " prm" << (k + 1);
         s << ") {\n" << f.body << "\n}\n";
     };
     std::function<int(int)> dependency = [&](int id) -> int {
@@ -182,11 +184,22 @@ static int sell_sweep_term(const vexb_expr &e, int *term) {
     return VEXB_OK;
 }
 
+// Whether a kernel passes a raw pointer to a user function (a VEXB_OP_TERM on a VEXB_TERM_PTR), whose body may write
+// through it: the kernel's loads then take the plain path, not the read-only one.
+static bool passes_pointers(const vexb_expr *const *es, int ncomp) {
+    for (int c = 0; c < ncomp; ++c)
+        for (int pc = 0; pc < es[c]->n_code; ++pc)
+            if (es[c]->code[pc].op == VEXB_OP_TERM && es[c]->term[es[c]->code[pc].arg].kind == VEXB_TERM_PTR) return true;
+    return false;
+}
+
 // Print instructions [from, to) of a normalised program as CUDA C onto the value stack `st`: one `const T rPC = ...;` per
 // instruction, whose semantics mirror csrc/expr_eval.cuh.  A TDEF prints `const T tK = <top>;` and names slot K tK; a
-// TREF pushes tnames[K], which is tK or the parameter that carries the value in (multi-expression kernels).
+// TREF pushes tnames[K], which is tK or the parameter that carries the value in (multi-expression kernels).  A pointer
+// argument pushes `(T *)tt.t[K].v.ptr`; a LOAD reads through the read-only path when `ldg` (nothing in the kernel
+// writes the array), else with a plain load.
 static void print_code(const vexb_expr &e, int from, int to, std::string (&tnames)[VEXB_MAX_TEMPS], std::ostream &s,
-                       std::vector<std::pair<std::string, int>> &st) {
+                       std::vector<std::pair<std::string, int>> &st, bool ldg = true) {
     for (int pc = from; pc < to; ++pc) {
         const vexb_instr &in = e.code[pc];
         const int op = in.op, t = in.type;
@@ -199,7 +212,16 @@ static void print_code(const vexb_expr &e, int from, int to, std::string (&tname
             continue;
         }
         if (op == VEXB_OP_TREF) { st.emplace_back(tnames[in.arg], t); continue; }
-        if (op == VEXB_OP_TERM) {
+        if (op == VEXB_OP_TERM && e.term[in.arg].kind == VEXB_TERM_PTR) {
+            st.emplace_back(std::string("(") + ctype(e.term[in.arg].dtype) + " *)tt.t[" + std::to_string(in.arg) + "].v.ptr", t);
+            continue;
+        }
+        if (op == VEXB_OP_LOAD) {                       // 0 outside [0, count): a guarded load never touches what its guard excludes
+            const std::string k = std::to_string(in.arg), idx = pop().first;
+            const std::string p = std::string("(const ") + ctype(t) + " *)tt.t[" + k + "].v.ptr + " + idx;
+            r << "(unsigned long long)" << idx << " < vexb_count(tt.t[" << k << "]) ? " << (ldg ? "__ldg(" + p + ")" : "*(" + p + ")")
+              << " : (" << ctype(t) << ")0";
+        } else if (op == VEXB_OP_TERM) {
             const vexb_term &tm = e.term[in.arg];
             const int k = in.arg;
             rt = tm.kind == VEXB_TERM_INDEX ? VEXB_U64 : tm.dtype;
@@ -322,7 +344,7 @@ static TempClasses temp_classes(const vexb_expr *const *es, int ncomp) {
                 continue;
             }
             key.push_back((char)in.op); key.push_back((char)in.type);
-            if (in.op == VEXB_OP_TERM) key.append(reinterpret_cast<const char *>(&e.term[in.arg]), sizeof(vexb_term));
+            if (in.op == VEXB_OP_TERM || in.op == VEXB_OP_LOAD) key.append(reinterpret_cast<const char *>(&e.term[in.arg]), sizeof(vexb_term));
             else if (in.op == VEXB_OP_TREF) key += "#" + std::to_string(tc.cls[c][in.arg]);
             else { key.push_back((char)(in.arg & 0xff)); key.push_back((char)(in.arg >> 8)); }
         }
@@ -340,6 +362,11 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
          "struct term_j { unsigned char kind, dtype, pad[6]; union { const void *ptr; double f64; float f32; int i32;"
          " unsigned int u32; long long i64; unsigned long long u64; } v; };\n"
          "struct terms_j { term_j t[" << VEXB_MAX_TERMS << "]; };\n";
+    bool loads = false;
+    for (int comp = 0; comp < ncomp; ++comp) loads = loads || expr_has_load(*es[comp]);
+    if (loads)                                          // the element count of a pointer terminal (pad[0..5], VEXB_TERM_PTR)
+        s << "__device__ __forceinline__ unsigned long long vexb_count(const term_j &t) {\n"
+             "  unsigned long long c = 0;\n  for (int b = 5; b >= 0; --b) c = c << 8 | t.pad[b];\n  return c;\n}\n";
     VEXB_TRY(emit_user_functions(es, ncomp, s));
     // sparse products used as terminals (VEXB_TERM_SPMV): one row function per terminal, specialised to the strip's format
     // -- hybrid ELL with the width as a literal (fully unrolled: all column/value loads, then all gathers of x, in
@@ -464,6 +491,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
              "  }\n  return sum;\n}\n";
     }
     const char *LT = ctype(lhs_dtype);
+    const bool ldg = !passes_pointers(es, ncomp);
     // Multi-expression kernels with temporaries: one function per class of temporaries (temp_classes), vexb_temp_g, which
     // takes the classes its definition reads as parameters g<j>; the kernel calls each once per element and passes the
     // values to the components, whose functions then start after their definitions.
@@ -479,7 +507,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
         for (int j : tc.reads[g]) s << ", const " << ctype(tc.type[j]) << " g" << j;
         s << ") {\n";
         std::vector<std::pair<std::string, int>> st;
-        print_code(e, tc.from[g], tc.to[g], tnames, s, st);
+        print_code(e, tc.from[g], tc.to[g], tnames, s, st, ldg);
         VEXB_CHECK(st.size() == 1, "internal: a temporary did not reduce to one value");
         s << "    return " << st.back().first << ";\n}\n";
     }
@@ -496,7 +524,7 @@ static int generate_elements(const vexb_expr *const *es, int ncomp, int lhs_dtyp
     }
     s << ") {\n";
     std::vector<std::pair<std::string, int>> st;        // (variable name, dtype)
-    print_code(e, multi_temps ? temp_prefix_length(e) : 0, e.n_code, tnames, s, st);
+    print_code(e, multi_temps ? temp_prefix_length(e) : 0, e.n_code, tnames, s, st, ldg);
     VEXB_CHECK(st.size() == 1, "internal: program did not reduce to one value");
     const std::string res = st.back().first; const int R = st.back().second;
     if (aop == VEXB_SET) {
@@ -1108,7 +1136,9 @@ extern "C" int vexb_function_register_ex(const char *name, int ret_dtype, int na
     for (const char *c = name; *c; ++c) VEXB_CHECK(isalnum((unsigned char)*c) || *c == '_', "'%s' is not an identifier", name);
     UserFunc f; f.name = name; f.ret = ret_dtype; f.body = body;
     for (int k = 0; k < nargs; ++k) {
-        VEXB_CHECK(arg_dtypes[k] >= VEXB_F64 && arg_dtypes[k] <= VEXB_U64, "bad type of argument %d", k);
+        // a value type, or VEXB_PTR(value type): a `T *` parameter that takes a VEXB_TERM_PTR terminal
+        const int base = is_ptr_type(arg_dtypes[k]) ? arg_dtypes[k] & ~VEXB_PTR(0) : arg_dtypes[k];
+        VEXB_CHECK(base >= VEXB_F64 && base <= VEXB_U64 && (arg_dtypes[k] == base || arg_dtypes[k] == VEXB_PTR(base)), "bad type of argument %d", k);
         f.args.push_back(arg_dtypes[k]);
     }
     if (preamble) f.preamble = preamble;

@@ -174,7 +174,7 @@ template <> __device__ __forceinline__ unsigned v_as<unsigned>(V v) { return (un
 template <> __device__ __forceinline__ long long v_as<long long>(V v) { return v.i; }
 template <> __device__ __forceinline__ unsigned long long v_as<unsigned long long>(V v) { return v.u; }
 
-template <int OP, class T, int U, bool TEMPS>
+template <int OP, class T, int U, bool EXT>
 __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constant__ vexb_expr e, int dtype, size_t n,
                                                              size_t index_offset, void *ws, T *result, PeerArgs pa) {
     const int rt = program_result_type(e);
@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constan
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int k = 0; k < U; ++k) { idx[k] = base + (size_t)k * blockDim.x + threadIdx.x; active[k] = idx[k] < n; }
-        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
+        eval_expr<U, EXT>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int k = 0; k < U; ++k) if (active[k]) acc[k].take(v_as<T>(convert(out[k], rt, dtype)));
     }
@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(256) reduce_interp_kernel(const __grid_constan
 // the GPUs).
 struct MultiOps { int n; int op[VEXB_MAX_COMBINED]; };
 
-template <class T, int U, bool TEMPS>
+template <class T, int U, bool EXT>
 __global__ void __launch_bounds__(256) reduce_multi_kernel(const __grid_constant__ vexb_expr e, int dtype, size_t n, size_t index_offset,
                                                             MultiOps ops, void *ws, size_t ws_stride, T *result, PeerArgs pa) {
     const int rt = program_result_type(e);
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(256) reduce_multi_kernel(const __grid_constant
         size_t idx[U]; bool active[U]; V out[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) { idx[u] = base + (size_t)u * blockDim.x + threadIdx.x; active[u] = idx[u] < n; }
-        eval_expr<U, TEMPS>(e, idx, active, index_offset, out);
+        eval_expr<U, EXT>(e, idx, active, index_offset, out);
 #pragma unroll
         for (int u = 0; u < U; ++u) if (active[u]) {
             const T v = v_as<T>(convert(out[u], rt, dtype));
@@ -240,6 +240,10 @@ __global__ void identity_kernel(T *result) {
 
 static const int kMaxBlocksPerSm = 16;
 
+// eval.jit != 0 (with eval.force_interp = 1 its default is 0): generated kernels may serve expressions that have no
+// hand-written form
+static bool jit_enabled() { return (param("eval.force_interp", 0) ? param("eval.jit", 0) : param("eval.jit", 2)) != 0; }
+
 template <int SH, class T>
 static void launch_rsweep(int op, int blocks, cudaStream_t st, const SweepArgs &a, size_t n, void *ws, void *res, const PeerArgs &pa) {
     switch (op) {
@@ -263,7 +267,7 @@ template <class T>
 static void launch_rinterp(int op, int blocks, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t off, void *ws, void *res, const PeerArgs &pa) {
     switch (op) {
 #define C(OP) case OP: \
-        if (expr_has_temps(e)) reduce_interp_kernel<OP, T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); \
+        if (expr_extended(e))  reduce_interp_kernel<OP, T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); \
         else                   reduce_interp_kernel<OP, T, 4, false><<<blocks, 256, 0, st>>>(e, dtype, n, off, ws, (T *)res, pa); \
         break;
         C(VEXB_SUM) C(VEXB_SUM_KAHAN) C(VEXB_MAX) C(VEXB_MIN) C(VEXB_MINMAX)
@@ -338,6 +342,12 @@ extern "C" int vexb_reduce_all(int dev, void *stream, const vexb_expr *expr, int
     const size_t cap = (size_t)sms * (size_t)bps;
     // user functions and inlined sparse products have no pre-compiled form: one kernel generated for the request (jit.cu)
     if (expr_has_call(e) || expr_has_product(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, 1, &op, false, cap, d_result, d_workspace, pa);
+    // loads through raw pointers: the generated kernel too unless eval.jit = 0 (its fold has the bits of reducing the
+    // expression's temporary), the interpreter when NVRTC cannot be loaded
+    if (expr_has_load(e) && jit_enabled()) {
+        const int s = jit_reduce(dev, st, e, dtype, n, index_offset, 1, &op, false, cap, d_result, d_workspace, pa);
+        if (s != VEXB_ERR_UNSUPPORTED) return s;
+    }
 
     if ((dtype == VEXB_F64 || dtype == VEXB_F32) && !param("eval.force_interp", 0)) {
         ShapeMatch m = match_shape(e, dtype);
@@ -429,7 +439,7 @@ extern "C" int vexb_cg_update_xp(int dev, void *stream, int dtype, size_t n, voi
 template <class T>
 static void launch_rmulti(int blocks, cudaStream_t st, const vexb_expr &e, int dtype, size_t n, size_t off, const vexb::MultiOps &ops,
                           void *ws, size_t stride, void *res, const PeerArgs &pa) {
-    if (vexb::expr_has_temps(e)) vexb::reduce_multi_kernel<T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
+    if (vexb::expr_extended(e))  vexb::reduce_multi_kernel<T, 4, true><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
     else                         vexb::reduce_multi_kernel<T, 4, false><<<blocks, 256, 0, st>>>(e, dtype, n, off, ops, ws, stride, (T *)res, pa);
 }
 
@@ -465,6 +475,10 @@ extern "C" int vexb_reduce_multi(int dev, void *stream, const vexb_expr *expr, i
     const int blocks = (int)(want < cap ? want : cap);
     cudaStream_t st = (cudaStream_t)stream;
     if (expr_has_call(e) || expr_has_product(e)) return jit_reduce(dev, st, e, dtype, n, index_offset, nops, mo.op, true, cap, d_result, d_workspace, pa);
+    if (expr_has_load(e) && jit_enabled()) {
+        const int s = jit_reduce(dev, st, e, dtype, n, index_offset, nops, mo.op, true, cap, d_result, d_workspace, pa);
+        if (s != VEXB_ERR_UNSUPPORTED) return s;
+    }
     switch (dtype) {
         case VEXB_F64: launch_rmulti<double>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
         case VEXB_F32: launch_rmulti<float>(blocks, st, e, dtype, n, index_offset, mo, d_workspace, stride, d_result, pa); break;
