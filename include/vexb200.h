@@ -804,6 +804,24 @@ int vexb_cg_update_r(int dev, void *stream, int dtype, size_t n, void *r, const 
 int vexb_cg_update_xp(int dev, void *stream, int dtype, size_t n, void *x, void *p, const void *r,
                       const void *d_rho, const void *d_pq, const void *d_rho_new);
 
+/* ------------------------------------------------------------------------
+ * Sort (vex::sort, vex::sort_by_key with vex::less / less_equal / greater / greater_equal, vexcl/sort.hpp).
+ * vexb_sort sorts n keys of `key_dtype` in place on one device slice, ascending (descending = 0) or descending, and
+ * moves the n values of `val_dtype` with them (vals = NULL and val_dtype = -1: keys only).  Stable in both directions.
+ * Floating keys: -0.0 equals +0.0, every NaN equals every other NaN and is greater than +inf; keys keep their bits.
+ * Asynchronous on `stream`; n < 2 launches nothing.  At most 2^31 - 1 elements.  d_workspace: device memory of at
+ * least vexb_sort_workspace_bytes(n, key_dtype, val_dtype) bytes (0 for n < 2, when it may be NULL).  Arguments are
+ * checked before anything touches the device (VEXB_ERR_INVALID).  Shape of the launches: csrc/sort.cu.
+ * vexb_sort_merge (host only) merges nparts sorted host runs, run p at [part[p] - part[0], part[p+1] - part[0]) of
+ * keys (and vals), into keys_out (and vals_out) in the same order, stably: equal keys keep their run order, then their
+ * order within the run.
+ * ---------------------------------------------------------------------- */
+int vexb_sort_workspace_bytes(size_t n, int key_dtype, int val_dtype, size_t *bytes);
+int vexb_sort(int dev, void *stream, void *keys, int key_dtype, void *vals, int val_dtype, size_t n, int descending,
+              void *d_workspace, size_t workspace_bytes);
+int vexb_sort_merge(int nparts, const size_t *part, const void *keys, int key_dtype, const void *vals, int val_dtype,
+                    int descending, void *keys_out, void *vals_out);
+
 #ifdef __cplusplus
 }
 #endif

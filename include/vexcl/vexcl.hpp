@@ -18,6 +18,7 @@
 #include "temporary.hpp"
 #include "vector_pointer.hpp"
 #include "reductor.hpp"
+#include "sort.hpp"
 #include "spmat.hpp"
 #include "spmat/ccsr.hpp"
 #include "stencil.hpp"

@@ -235,6 +235,9 @@ def lib():
         "vexb_reduce_multi": ([i, vp, P(Expr), i, sz, sz, i, P(i), vp, vp, vp], i),
         "vexb_cg_update_r": ([i, vp, i, sz, vp, vp, vp, vp, vp, vp, vp], i),
         "vexb_cg_update_xp": ([i, vp, i, sz, vp, vp, vp, vp, vp, vp], i),
+        "vexb_sort_workspace_bytes": ([sz, i, i, P(sz)], i),
+        "vexb_sort": ([i, vp, vp, i, vp, i, sz, i, vp, sz], i),
+        "vexb_sort_merge": ([i, P(sz), vp, i, vp, i, i, vp, vp], i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)          # AttributeError here == the library does not export a declared symbol

@@ -1844,3 +1844,56 @@ def assign_multi(lhs, rhs, op: int = L.SET) -> bool:
     for v, t in zip(lhs, tmp):
         v._assign(op, t)
     return False
+
+
+# ------------------------------------------------------------------------------------------- sort
+def _sort(keys: vector, vals: Optional[vector], descending: bool):
+    """vexb_sort on every slice (on its own stream, workspace allocated per call and part), then, with several parts,
+    the stable host merge of the sorted slices (vexb_sort_merge), written back: vex::sort's sort_sink (sort.hpp:2070-2116)."""
+    ctx = keys.ctx
+    if vals is not None and (vals.ctx is not ctx or vals.n != keys.n or not np.array_equal(vals.part, keys.part)):
+        raise ValueError("Keys and values span different devices")
+    if ctx.is_distributed:
+        raise ValueError("sort needs every part of the vector in this process")
+    lib = L.lib()
+    vdt = -1 if vals is None else vals.dtype
+    for k in ctx.local:
+        n = keys.part_size(k)
+        if n == 0:
+            continue
+        nb = C.c_size_t()
+        L.check(lib.vexb_sort_workspace_bytes(n, keys.dtype, vdt, C.byref(nb)))
+        ws = C.c_void_p()
+        if nb.value:
+            L.check(lib.vexb_malloc(ctx.devs[k], nb.value, C.byref(ws)))
+        try:
+            L.check(lib.vexb_sort(ctx.devs[k], ctx.streams[k], keys.bufs[k], keys.dtype, None if vals is None else vals.bufs[k],
+                                  vdt, n, int(bool(descending)), ws, nb.value))
+        finally:
+            if ws.value:
+                lib.vexb_free(ctx.devs[k], ws)
+    if ctx.nparts == 1:
+        return
+    hk = keys.read()
+    ok = np.empty_like(hk)
+    hv = ov = None
+    if vals is not None:
+        hv = vals.read()
+        ov = np.empty_like(hv)
+    part = (C.c_size_t * (ctx.nparts + 1))(*[int(p) for p in keys.part])
+    L.check(lib.vexb_sort_merge(ctx.nparts, part, hk.ctypes.data, keys.dtype, None if hv is None else hv.ctypes.data, vdt,
+                                int(bool(descending)), ok.ctypes.data, None if ov is None else ov.ctypes.data))
+    keys.write(ok)
+    if vals is not None:
+        vals.write(ov)
+
+
+def sort(keys: vector, descending: bool = False):
+    """vex::sort(keys[, vex::less / vex::greater]): a stable sort in place, ascending or descending.  Floating keys: -0.0
+    equals +0.0, NaNs equal each other and follow +inf (numpy's and torch's order)."""
+    _sort(keys, None, descending)
+
+
+def sort_by_key(keys: vector, vals: vector, descending: bool = False):
+    """vex::sort_by_key(keys, vals[, comparator]): sort keys stably in place and move vals with them."""
+    _sort(keys, vals, descending)
