@@ -822,6 +822,35 @@ int vexb_sort(int dev, void *stream, void *keys, int key_dtype, void *vals, int 
 int vexb_sort_merge(int nparts, const size_t *part, const void *keys, int key_dtype, const void *vals, int val_dtype,
                     int descending, void *keys_out, void *vals_out);
 
+/* ------------------------------------------------------------------------
+ * Scans (vex::inclusive_scan, vex::exclusive_scan, vexcl/scan.hpp), scans by key (vex::inclusive_scan_by_key,
+ * vex::exclusive_scan_by_key, vexcl/scan_by_key.hpp) and vex::reduce_by_key (vexcl/reduce_by_key.hpp) of one device
+ * slice, with `+` on the values and `==` on the keys.  Integer sums wrap; every float add is rounded on its own, in an
+ * order that depends on n only (csrc/scan.cu).  A run is a maximal range of keys equal under ==: -0.0 and +0.0 share
+ * one, every NaN key is a run of its own.
+ * vexb_scan: out[i] = in[0] + ... + in[i] (inclusive; h_init is not read) or, exclusive, out[0] = *h_init with its own
+ * bits and out[i] = *h_init + in[0] + ... + in[i-1].  in == out scans in place.
+ * vexb_scan_by_key: the same within every run of keys; an exclusive scan starts every run at *h_init.  ivals == ovals
+ * scans in place; keys must not be ovals.
+ * vexb_reduce_by_key_count runs the first two of the three launches and returns the number of runs in *nruns (one
+ * device-to-host read; it waits for the stream); vexb_reduce_by_key_write, with the same arguments and workspace, then
+ * writes the last key of run j to okeys[j] and the sum of its values to ovals[j].  The outputs must not alias the
+ * inputs or each other.
+ * h_init: one element of the value dtype on the host; NULL reads as zero.  Asynchronous on `stream` (apart from
+ * vexb_reduce_by_key_count); n = 0 launches nothing.  At most 2^31 - 1 elements.  d_workspace: device memory of at least
+ * vexb_scan_workspace_bytes(n, val_dtype) bytes (0 for n = 0, when it may be NULL).  Arguments are checked before
+ * anything touches the device (VEXB_ERR_INVALID).
+ * ---------------------------------------------------------------------- */
+int vexb_scan_workspace_bytes(size_t n, int val_dtype, size_t *bytes);
+int vexb_scan(int dev, void *stream, const void *in, void *out, int dtype, size_t n, int exclusive, const void *h_init,
+              void *d_workspace, size_t workspace_bytes);
+int vexb_scan_by_key(int dev, void *stream, const void *keys, int key_dtype, const void *ivals, void *ovals, int val_dtype,
+                     size_t n, int exclusive, const void *h_init, void *d_workspace, size_t workspace_bytes);
+int vexb_reduce_by_key_count(int dev, void *stream, const void *ikeys, int key_dtype, const void *ivals, int val_dtype,
+                             size_t n, void *d_workspace, size_t workspace_bytes, size_t *nruns);
+int vexb_reduce_by_key_write(int dev, void *stream, const void *ikeys, int key_dtype, const void *ivals, int val_dtype,
+                             size_t n, void *okeys, void *ovals, void *d_workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,9 @@
 #include "vector_pointer.hpp"
 #include "reductor.hpp"
 #include "sort.hpp"
+#include "scan.hpp"
+#include "scan_by_key.hpp"
+#include "reduce_by_key.hpp"
 #include "spmat.hpp"
 #include "spmat/ccsr.hpp"
 #include "stencil.hpp"

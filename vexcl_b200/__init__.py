@@ -12,7 +12,8 @@ from .api import (Context, vector, Reductor, SpMat, SpMatCCSR, BlockMatrix, Comp
                   sin, cos, tan, asin, acos, atan, sinh, cosh, tanh, exp, exp2, log, log2, log10, sqrt, rsqrt,
                   cbrt, fabs, floor, ceil, round_, trunc, pow_, atan2, fmod, hypot, fmin, fmax, fma, make_inline, InlineSpMV, assign_multi,
                   UserFunction, push_program_header, pop_program_header, program_header, make_temp, Temp,
-                  raw_pointer, deref, ptr, Pointer, Load, sort, sort_by_key)
+                  raw_pointer, deref, ptr, Pointer, Load, sort, sort_by_key,
+                  inclusive_scan, exclusive_scan, inclusive_scan_by_key, exclusive_scan_by_key, reduce_by_key)
 
 
 def set_param(name: str, value: int):

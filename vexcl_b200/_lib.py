@@ -238,6 +238,11 @@ def lib():
         "vexb_sort_workspace_bytes": ([sz, i, i, P(sz)], i),
         "vexb_sort": ([i, vp, vp, i, vp, i, sz, i, vp, sz], i),
         "vexb_sort_merge": ([i, P(sz), vp, i, vp, i, i, vp, vp], i),
+        "vexb_scan_workspace_bytes": ([sz, i, P(sz)], i),
+        "vexb_scan": ([i, vp, vp, vp, i, sz, i, vp, vp, sz], i),
+        "vexb_scan_by_key": ([i, vp, vp, i, vp, vp, i, sz, i, vp, vp, sz], i),
+        "vexb_reduce_by_key_count": ([i, vp, vp, i, vp, i, sz, vp, sz, P(sz)], i),
+        "vexb_reduce_by_key_write": ([i, vp, vp, i, vp, i, sz, vp, vp, vp, sz], i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)          # AttributeError here == the library does not export a declared symbol

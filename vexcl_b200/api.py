@@ -1897,3 +1897,173 @@ def sort(keys: vector, descending: bool = False):
 def sort_by_key(keys: vector, vals: vector, descending: bool = False):
     """vex::sort_by_key(keys, vals[, comparator]): sort keys stably in place and move vals with them."""
     _sort(keys, vals, descending)
+
+
+# ------------------------------------------------------------------------------------------- scans
+def _scan_identity(np_dtype):
+    """The exact identity of the element type's add: -0.0 for floats (-0.0 + x == x, also for x = +0.0), 0 otherwise."""
+    return np_dtype.type(-0.0) if np_dtype.kind == "f" else np_dtype.type(0)
+
+
+def _as_element(value, np_dtype) -> np.ndarray:
+    """`value` as one element of np_dtype; integers wrap, as the C++ conversion does."""
+    a = np.asarray(value)
+    if np_dtype.kind in "iu" and a.dtype.kind in "iu":
+        return np.array([int(a) % (1 << (8 * np_dtype.itemsize))], dtype=np.uint64).astype(np_dtype)
+    return np.array([a], dtype=np_dtype)
+
+
+def _scan_workspace(ctx, k, n, dtype):
+    lib = L.lib()
+    nb = C.c_size_t()
+    L.check(lib.vexb_scan_workspace_bytes(n, dtype, C.byref(nb)))
+    ws = C.c_void_p()
+    if nb.value:
+        L.check(lib.vexb_malloc(ctx.devs[k], nb.value, C.byref(ws)))
+    return ws, nb.value
+
+
+def _element(vec: vector, k: int, i: int):
+    """Element i of slice k (a blocking one-element read)."""
+    out = np.empty(1, dtype=vec.np_dtype)
+    es = vec.np_dtype.itemsize
+    L.check(L.lib().vexb_d2h(vec.ctx.devs[k], out.ctypes.data, C.c_void_p(vec.bufs[k].value + i * es), es, vec.ctx.streams[k], 1))
+    return out[0]
+
+
+def _add_to_slice(vec: vector, k: int, value):
+    """Slice k of vec += value, one launch of the expression path."""
+    low = _Lowering(k, vec.part_start(k))
+    low.size = vec.n
+    low.target = vec
+    low.sweep = None
+    low.see(vec)
+    low.lower(Scalar(value, vec.dtype))
+    L.check(L.lib().vexb_eval(vec.ctx.devs[k], vec.ctx.streams[k], vec.bufs[k], vec.dtype, L.ADD, C.byref(low.e),
+                              vec.part_size(k), vec.part_start(k)))
+
+
+def _scan(inp: vector, out: vector, init, exclusive: bool):
+    """vexb_scan on every slice; with several parts, the local totals are folded on the host in the element type and
+    each carry is added to its slice (scan.hpp:426-518), with init counted once: only the first non-empty slice starts
+    at init, the others at the identity."""
+    ctx = inp.ctx
+    if out.ctx is not ctx or out.dtype != inp.dtype or out.n != inp.n or not np.array_equal(out.part, inp.part):
+        raise ValueError("Incompatible partitioning")
+    if ctx.is_distributed:
+        raise ValueError("scan needs every part of the vector in this process")
+    lib = L.lib()
+    dt = inp.np_dtype
+    first = _as_element(init, dt)
+    ident = np.array([_scan_identity(dt)], dtype=dt)
+    several = ctx.nparts > 1
+    # an exclusive scan in place overwrites each slice's last input, which its carry needs: read those first
+    last_in = {k: _element(inp, k, inp.part_size(k) - 1) for k in ctx.local if several and exclusive and inp.part_size(k)}
+    started = False
+    for k in ctx.local:
+        n = inp.part_size(k)
+        if n == 0:
+            continue
+        ws, nb = _scan_workspace(ctx, k, n, inp.dtype)
+        try:
+            L.check(lib.vexb_scan(ctx.devs[k], ctx.streams[k], inp.bufs[k], out.bufs[k], inp.dtype, n, int(bool(exclusive)),
+                                  (ident if started else first).ctypes.data, ws, nb))
+        finally:
+            if ws.value:
+                lib.vexb_free(ctx.devs[k], ws)
+        started = True
+    if not several:
+        return
+    carry = None
+    with np.errstate(over="ignore"):
+        for k in ctx.local:
+            n = out.part_size(k)
+            if n == 0:
+                continue
+            total = _element(out, k, n - 1)
+            if exclusive:
+                total = dt.type(total + last_in[k])
+            if carry is None:
+                carry = total
+            else:
+                _add_to_slice(out, k, carry)
+                carry = dt.type(carry + total)
+
+
+def inclusive_scan(inp: vector, out: vector, init=0):
+    """vex::inclusive_scan(in, out[, init]): out[i] = in[0] + ... + in[i].  `init` is not read, as in the reference,
+    whose kernels ignore it for inclusive scans.  out may be inp.  Integer sums wrap; every float add is rounded."""
+    _scan(inp, out, init, False)
+
+
+def exclusive_scan(inp: vector, out: vector, init=0):
+    """vex::exclusive_scan(in, out[, init]): out[0] = init (its own bits), out[i] = init + in[0] + ... + in[i-1].  out
+    may be inp.  On several parts init is counted once (the reference adds it once per part)."""
+    _scan(inp, out, init, True)
+
+
+def _by_key_checks(keys: vector, ivals: vector, what: str):
+    if keys.ctx.nparts != 1 or ivals.ctx.nparts != 1:
+        raise ValueError(f"{what} is only supported for single device contexts")
+    if keys.ctx.is_distributed:
+        raise ValueError(f"{what} is only supported for single device contexts")
+    if keys.n != ivals.n:
+        raise ValueError("keys and values should have same size")
+
+
+def _scan_by_key(keys: vector, ivals: vector, ovals: vector, init, exclusive: bool):
+    _by_key_checks(keys, ivals, "scan_by_key")
+    if ovals.ctx.nparts != 1 or ovals.n != ivals.n or ovals.dtype != ivals.dtype:
+        raise ValueError("input and output should have same size")
+    ctx = keys.ctx
+    k = ctx.local[0]
+    n = keys.n
+    if n == 0:
+        return
+    if ovals.bufs[k].value == keys.bufs[k].value:
+        raise ValueError("keys and ovals are the same buffer")
+    lib = L.lib()
+    first = _as_element(init, ivals.np_dtype)
+    ws, nb = _scan_workspace(ctx, k, n, ivals.dtype)
+    try:
+        L.check(lib.vexb_scan_by_key(ctx.devs[k], ctx.streams[k], keys.bufs[k], keys.dtype, ivals.bufs[k], ovals.bufs[k],
+                                     ivals.dtype, n, int(bool(exclusive)), first.ctypes.data, ws, nb))
+    finally:
+        if ws.value:
+            lib.vexb_free(ctx.devs[k], ws)
+
+
+def inclusive_scan_by_key(keys: vector, ivals: vector, ovals: vector, init=0):
+    """vex::inclusive_scan_by_key(keys, ivals, ovals[, init]): the inclusive sum within every run of keys equal under
+    == (-0.0 and +0.0 share a run, every NaN key is a run of its own).  `init` is not read, as in the reference.
+    ovals may be ivals.  One-part vectors only."""
+    _scan_by_key(keys, ivals, ovals, init, False)
+
+
+def exclusive_scan_by_key(keys: vector, ivals: vector, ovals: vector, init=0):
+    """vex::exclusive_scan_by_key(keys, ivals, ovals[, init]): the exclusive sum within every run of keys, each run
+    starting at init.  ovals may be ivals.  One-part vectors only."""
+    _scan_by_key(keys, ivals, ovals, init, True)
+
+
+def reduce_by_key(ikeys: vector, ivals: vector):
+    """vex::reduce_by_key(ikeys, ivals, okeys, ovals): (okeys, ovals) as new vectors with one element per run of keys
+    equal under ==: okeys[j] holds the bits of the last key of run j and ovals[j] the sum of its values.  One-part
+    vectors only."""
+    _by_key_checks(ikeys, ivals, "reduce_by_key")
+    ctx = ikeys.ctx
+    k = ctx.local[0]
+    n = ikeys.n
+    lib = L.lib()
+    ws, nb = _scan_workspace(ctx, k, n, ivals.dtype)
+    try:
+        runs = C.c_size_t()
+        L.check(lib.vexb_reduce_by_key_count(ctx.devs[k], ctx.streams[k], ikeys.bufs[k], ikeys.dtype, ivals.bufs[k],
+                                             ivals.dtype, n, ws, nb, C.byref(runs)))
+        okeys, ovals = vector(ctx, runs.value, ikeys.np_dtype), vector(ctx, runs.value, ivals.np_dtype)
+        L.check(lib.vexb_reduce_by_key_write(ctx.devs[k], ctx.streams[k], ikeys.bufs[k], ikeys.dtype, ivals.bufs[k],
+                                             ivals.dtype, n, okeys.bufs[k], ovals.bufs[k], ws, nb))
+    finally:
+        if ws.value:
+            lib.vexb_free(ctx.devs[k], ws)
+    return okeys, ovals
